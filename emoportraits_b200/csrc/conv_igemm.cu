@@ -443,18 +443,23 @@ static int pick_box(int dim, int want) {
   return b < 1 ? 1 : b;
 }
 
-}  // namespace emo
+// What emo_conv_igemm runs for one descriptor: the kernel parameters (tiles, N tile, k-chunk, pipeline depths, split-K,
+// accumulation chunk), the kernel form, the grid, the shared-memory size and the launches that finish the convolution.
+struct ConvPlan {
+  ConvKParams p;
+  int NP, KC, f16, ps, kh_eff;
+  int kernel;  // EMO_CONV_KERNEL_*
+  int grid;
+  int finish;  // EMO_CONV_FINISH_*
+  size_t smem_bytes;
+};
 
-using namespace emo;
-
-#ifdef EMO_CONV_DEBUG
-extern "C" int emo_debug_conv_stamps(unsigned long long* host160x16) {
-  return cudaMemcpyFromSymbol(host160x16, g_conv_stamps, sizeof(unsigned long long) * 160 * 16) == cudaSuccess ? 0 : -2;
-}
-#endif
-
-extern "C" int emo_conv_igemm(const emo_conv_desc* d, void* stream_) {
-  cudaStream_t stream = (cudaStream_t)stream_;
+// Checks the descriptor and plans the launch for a device of `sm_count` SMs.  Host arithmetic only (no CUDA call): emo_conv_plan
+// reports the same plan without a device.
+static int plan_conv(const emo_conv_desc* d, int sm_count, ConvPlan* plan) {
+  EMO_REQUIRE(plan && sm_count >= 1, "emo_conv_igemm: bad plan arguments (sm_count=%d)", sm_count);
+  memset(plan, 0, sizeof(*plan));
+  ConvKParams& p = plan->p;
   EMO_REQUIRE(d && d->a_hi && d->a_lo && d->w_hi && d->w_lo && d->out, "emo_conv_igemm: null pointer");
   EMO_REQUIRE(d->Cin % 32 == 0, "emo_conv_igemm: Cin=%d must be a multiple of 32 (use emo_conv_direct)", d->Cin);
   EMO_REQUIRE(d->Cout_pad % 16 == 0 && d->Cout <= d->Cout_pad, "emo_conv_igemm: Cout_pad=%d must be a multiple of 16 >= Cout", d->Cout_pad);
@@ -471,8 +476,6 @@ extern "C" int emo_conv_igemm(const emo_conv_desc* d, void* stream_) {
   const bool vec_ok = (d->Cout % 4 == 0);
   EMO_REQUIRE(vec_ok || d->Cout < 16, "emo_conv_igemm: Cout=%d must be a multiple of 4 (or < 16)", d->Cout);
 
-  PFN_cuTensorMapEncodeTiled encode = get_encode();
-  if (!encode) { set_error("emo_conv_igemm: cuTensorMapEncodeTiled entry point unavailable"); return EMO_ERR_CUDA; }
   const int NP = d->a_lo2 ? 3 : 2;
   EMO_REQUIRE((d->a_lo2 == nullptr) == (d->w_lo2 == nullptr), "emo_conv_igemm: a_lo2 and w_lo2 must be given together");
   // sub-pixel mode: the descriptor describes conv3x3(pad 1)(nearest_x2(input)) with the input given at LOW resolution and
@@ -497,14 +500,7 @@ extern "C" int emo_conv_igemm(const emo_conv_desc* d, void* stream_) {
   for (int cand = kMaxBN; cand >= 16; cand -= 16)
     if (d->Cout_pad % cand == 0) { BN = cand; break; }
   EMO_REQUIRE(BN > 0, "emo_conv_igemm: no N tile for Cout_pad=%d", d->Cout_pad);
-  int sm_count = 132, cur_dev = 0;
-  {
-    cudaGetDevice(&cur_dev);
-    cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, cur_dev);
-  }
 
-  ConvKParams p;
-  memset(&p, 0, sizeof(p));
   p.N = d->N; p.Dout = d->Dout; p.Hout = gH; p.Wout = gW; p.Cout = d->Cout;
   p.oH = d->Hout; p.oW = d->Wout;
   p.kd = d->kd; p.kh = ps ? 2 : d->kh; p.kw = ps ? 2 : d->kw; p.sd = d->sd; p.sh = d->sh; p.sw = d->sw;
@@ -607,6 +603,70 @@ extern "C" int emo_conv_igemm(const emo_conv_desc* d, void* stream_) {
     p.flush = target / mmas_per_kstep < 1 ? 1 : target / mmas_per_kstep;
   }
   const size_t smem_bytes = ring_bytes + tail_bytes + 1024;
+  const int total_tiles = p.m_tiles * p.n_tiles * p.ksplit;
+  const int grid = total_tiles < sm_count ? total_tiles : sm_count;
+  const long long per_n = (long long)d->Dout * d->Hout * d->Wout * d->Cout;
+  const emo_apply_desc* post = d->post;
+  if (ksplit > 1 && post && post->up == 1 && !d->out_nchw && !d->post_add && per_n <= (long long)kPostCluster * kPostThreads * kPostMaxV &&
+      d->Cout <= kPostThreads && kPostThreads % d->Cout == 0 && (!post->stats || (post->G <= 64 && d->Cout % post->G == 0)))
+    plan->finish = EMO_CONV_FINISH_POST;
+  else if (ksplit > 1)
+    plan->finish = post ? EMO_CONV_FINISH_FINALIZE_APPLY : EMO_CONV_FINISH_FINALIZE;
+  else
+    plan->finish = post ? EMO_CONV_FINISH_APPLY : EMO_CONV_FINISH_NONE;
+  plan->NP = NP; plan->KC = KC; plan->f16 = f16; plan->ps = ps; plan->kh_eff = kh_eff;
+  plan->kernel = f16 ? (KC == 64 ? EMO_CONV_KERNEL_F16_KC64 : EMO_CONV_KERNEL_F16_KC32)
+                 : ps ? EMO_CONV_KERNEL_UPCONV_KC64
+                 : NP == 3 ? (KC == 64 ? EMO_CONV_KERNEL_BF16X3_KC64 : EMO_CONV_KERNEL_BF16X3_KC32)
+                           : (KC == 64 ? EMO_CONV_KERNEL_BF16X2_KC64 : EMO_CONV_KERNEL_BF16X2_KC32);
+  plan->grid = grid;
+  plan->smem_bytes = smem_bytes;
+  return EMO_OK;
+}
+
+}  // namespace emo
+
+using namespace emo;
+
+#ifdef EMO_CONV_DEBUG
+extern "C" int emo_debug_conv_stamps(unsigned long long* host160x16) {
+  return cudaMemcpyFromSymbol(host160x16, g_conv_stamps, sizeof(unsigned long long) * 160 * 16) == cudaSuccess ? 0 : -2;
+}
+#endif
+
+extern "C" int emo_conv_plan(const emo_conv_desc* d, int sm_count, emo_conv_plan_info* out) {
+  EMO_REQUIRE(out, "emo_conv_plan: null output");
+  ConvPlan plan;
+  const int rc = plan_conv(d, sm_count, &plan);
+  if (rc) return rc;
+  const ConvKParams& p = plan.p;
+  memset(out, 0, sizeof(*out));
+  out->kernel = plan.kernel; out->KC = plan.KC; out->NP = plan.NP; out->fp16 = plan.f16;
+  out->BN = p.BN; out->ksplit = p.ksplit; out->yreuse = p.yreuse; out->sa = p.sa; out->sb = p.sb;
+  out->stages = p.stages; out->flush = p.flush;
+  out->tw = p.tw; out->th = p.th; out->td = p.td;
+  out->m_tiles = p.m_tiles; out->n_tiles = p.n_tiles; out->grid = plan.grid; out->finish = plan.finish;
+  return EMO_OK;
+}
+
+extern "C" int emo_conv_igemm(const emo_conv_desc* d, void* stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  int sm_count = 132, cur_dev = 0;
+  {
+    cudaGetDevice(&cur_dev);
+    cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, cur_dev);
+  }
+  ConvPlan plan;
+  {
+    const int rc = plan_conv(d, sm_count, &plan);
+    if (rc) return rc;
+  }
+  PFN_cuTensorMapEncodeTiled encode = get_encode();
+  if (!encode) { set_error("emo_conv_igemm: cuTensorMapEncodeTiled entry point unavailable"); return EMO_ERR_CUDA; }
+  const ConvKParams& p = plan.p;
+  const int NP = plan.NP, KC = plan.KC, f16 = plan.f16, ps = plan.ps, kh_eff = plan.kh_eff, BN = p.BN, ksplit = p.ksplit;
+  const int grid = plan.grid;
+  const size_t smem_bytes = plan.smem_bytes;
 
   // ---- tensor maps ----
   TMaps tm;
@@ -640,8 +700,6 @@ extern "C" int emo_conv_igemm(const emo_conv_desc* d, void* stream_) {
     }
   }
 
-  const int total_tiles = p.m_tiles * p.n_tiles * p.ksplit;
-  const int grid = total_tiles < sm_count ? total_tiles : sm_count;
   cudaError_t e;
 #define EMO_LAUNCH_CONV(KERNEL_, KC_, NP_)                                                                                 \
   do {                                                                                                                    \
@@ -669,10 +727,8 @@ extern "C" int emo_conv_igemm(const emo_conv_desc* d, void* stream_) {
     else EMO_LAUNCH_CONV(conv_igemm_kernel, 32, 2);
   }
 #undef EMO_LAUNCH_CONV
-  const long long per_n = (long long)d->Dout * d->Hout * d->Wout * d->Cout;
   const emo_apply_desc* post = d->post;
-  if (ksplit > 1 && post && post->up == 1 && !d->out_nchw && !d->post_add && per_n <= (long long)kPostCluster * kPostThreads * kPostMaxV &&
-      d->Cout <= kPostThreads && kPostThreads % d->Cout == 0 && (!post->stats || (post->G <= 64 && d->Cout % post->G == 0))) {
+  if (plan.finish == EMO_CONV_FINISH_POST) {
     // small split-K layer with a post-op: one cluster per sample finishes the convolution, normalises, activates and writes the
     // next convolution's operand planes (splitk_post_kernel)
     PostParams f;

@@ -69,6 +69,17 @@ class ConvDesc(C.Structure):
                 ("operand_fp16", c_int), ("out_scale", c_float), ("post", c_void_p)]
 
 
+class ConvPlanInfo(C.Structure):
+    _fields_ = [("kernel", c_int), ("KC", c_int), ("NP", c_int), ("fp16", c_int), ("BN", c_int), ("ksplit", c_int),
+                ("yreuse", c_int), ("sa", c_int), ("sb", c_int), ("stages", c_int), ("flush", c_int), ("tw", c_int),
+                ("th", c_int), ("td", c_int), ("m_tiles", c_int), ("n_tiles", c_int), ("grid", c_int), ("finish", c_int)]
+
+
+# emo_conv_plan_info.kernel and .finish (EMO_CONV_KERNEL_* / EMO_CONV_FINISH_*)
+CONV_KERNELS = ("conv<64,2>", "conv<32,2>", "conv<64,3>", "conv<32,3>", "f16<64,2>", "f16<32,2>", "ps<64,2>")
+CONV_FINISH = ("none", "finalize", "post", "finalize+apply", "apply")
+
+
 class ConvDirectDesc(C.Structure):
     _fields_ = [("x", c_void_p), ("N", c_int), ("Hin", c_int), ("Win", c_int), ("Cin_pad", c_int), ("w", c_void_p),
                 ("Cout", c_int), ("kh", c_int), ("kw", c_int), ("stride", c_int), ("pad", c_int), ("Hout", c_int),
@@ -106,6 +117,7 @@ SYMBOLS = {
     "emo_apply": (c_int, [C.POINTER(ApplyDesc), c_void_p]),
     "emo_gn_head": (c_int, [C.POINTER(GnHeadDesc), c_void_p]),
     "emo_conv_igemm": (c_int, [C.POINTER(ConvDesc), c_void_p]),
+    "emo_conv_plan": (c_int, [C.POINTER(ConvDesc), c_int, C.POINTER(ConvPlanInfo)]),
     "emo_conv_direct": (c_int, [C.POINTER(ConvDirectDesc), c_void_p]),
     "emo_linear": (c_int, [C.POINTER(LinearDesc), c_void_p]),
     "emo_upsample_trilinear": (c_int, [C.POINTER(ResampleDesc), c_void_p]),

@@ -437,19 +437,13 @@ def set_conv_profiler(p: Optional[ConvProfiler]):
     _conv_profiler = p
 
 
-def conv_igemm(a: Split, w: PackedConvWeight, stride=(1, 1, 1), pad=None, bias=None, residual=None, res_shift: int = 0,
-               act: int = ACT_NONE, post_add=None, out_nchw: bool = False, stats: Optional[torch.Tensor] = None,
-               G: int = 32, out: Optional[torch.Tensor] = None, acc_chunk_mmas: int = 0, split_k: bool = True,
-               upconv: bool = False, post: Optional[dict] = None):
-    """upconv=True: `a` holds the LOW-resolution planes and `w` a pack_upconv_weight(): the result is
-    conv3x3(pad 1)(nearest_x2(a)) at (2H, 2W), evaluated in sub-pixel form (see emo_conv_desc.upconv).
-    post = dict(<arguments of apply()>): the elementwise pass that follows the convolution (GroupNorm / affine + residual +
-    activation -> fp32 and/or operand planes; a `gn` post-op normalises with this convolution's `stats`).  Small split-K layers
-    run it inside the finalize step (one launch instead of three, emo_conv_desc.post).  With `post` the call returns what
-    apply() would return for it; the raw convolution output is then an internal scratch tensor."""
+def _conv_desc(a: Split, w: PackedConvWeight, stride, pad, bias, residual, res_shift, act, post_add, out_nchw, stats, G, out,
+               acc_chunk_mmas, split_k, upconv, post):
+    """emo_conv_desc of one conv_igemm() call (with its freshly allocated output unless `out` is given), the value the call
+    returns, the ctypes objects the descriptor points to, and the profiler label / algorithmic flops / MMA passes."""
     N, Di, Hi, Wi, Ci = a.shape
     assert Ci == w.cin, (Ci, w.cin)
-    ws = None if (L.DRY_RUN or not split_k) else _splitk_workspace(a.hi.device)
+    ws = None if not split_k else _splitk_workspace(a.hi.device)
     three = a.lo2 is not None
     assert not three or w.lo2 is not None, "3-plane activations need 3-plane weights (pack_conv_weight(planes=3))"
     assert a.f16 == w.f16, "fp16-plane activations need fp16-plane weights (pack_conv_weight(planes='h2')) and vice versa"
@@ -470,7 +464,7 @@ def conv_igemm(a: Split, w: PackedConvWeight, stride=(1, 1, 1), pad=None, bias=N
                    G if stats is not None else 0, _p(a.lo2) if three else None, _p(w.lo2) if three else None,
                    acc_chunk_mmas or w.acc_chunk, _p(ws), ws.numel() if ws is not None else 0, 1 if upconv else 0,
                    1 if a.f16 else 0, 1.0 / (a.scale * w.scale) if a.f16 else 0.0, None)
-    post_ret = None
+    ret, pd = out, None
     if post is not None:
         assert not out_nchw and not upconv, "post-op: channels-last output of a plain convolution"
         pkw = dict(post)
@@ -479,21 +473,54 @@ def conv_igemm(a: Split, w: PackedConvWeight, stride=(1, 1, 1), pad=None, bias=N
         pd, pout, psp = _apply_desc(None, (N, Do, Ho, Wo, w.cout), a.hi.device, **pkw)
         d.post = C.cast(C.pointer(pd), C.c_void_p)
         wf, wsp = pkw.get("want_f32", False), pkw.get("want_split", True)
-        post_ret = (pout, psp) if (wf and wsp) else (pout if wf else psp)
+        ret = (pout, psp) if (wf and wsp) else (pout if wf else psp)
+    # algorithmic flops of the convolution being computed; MMA passes actually issued per algorithmic product
+    # (sub-pixel mode issues 4 of the 9 taps)
+    prof = (2.0 * N * Do * Ho * Wo * w.cout * Ci * kd * kh * kw, (6 if three else 3) * (4.0 / 9.0 if upconv else 1.0),
+            f"{N}x{Di}x{Hi}x{Wi}x{Ci}->{w.cout} k{kd}{kh}{kw} s{stride[1]} p{'h2' if a.f16 else (3 if three else 2)}"
+            + (" up2-subpixel" if upconv else ""))
+    return d, ret, pd, prof
+
+
+def conv_igemm(a: Split, w: PackedConvWeight, stride=(1, 1, 1), pad=None, bias=None, residual=None, res_shift: int = 0,
+               act: int = ACT_NONE, post_add=None, out_nchw: bool = False, stats: Optional[torch.Tensor] = None,
+               G: int = 32, out: Optional[torch.Tensor] = None, acc_chunk_mmas: int = 0, split_k: bool = True,
+               upconv: bool = False, post: Optional[dict] = None):
+    """upconv=True: `a` holds the LOW-resolution planes and `w` a pack_upconv_weight(): the result is
+    conv3x3(pad 1)(nearest_x2(a)) at (2H, 2W), evaluated in sub-pixel form (see emo_conv_desc.upconv).
+    post = dict(<arguments of apply()>): the elementwise pass that follows the convolution (GroupNorm / affine + residual +
+    activation -> fp32 and/or operand planes; a `gn` post-op normalises with this convolution's `stats`).  Small split-K layers
+    run it inside the finalize step (one launch instead of three, emo_conv_desc.post).  With `post` the call returns what
+    apply() would return for it; the raw convolution output is then an internal scratch tensor."""
+    d, ret, _pd, prof = _conv_desc(a, w, stride, pad, bias, residual, res_shift, act, post_add, out_nchw, stats, G, out,
+                                   acc_chunk_mmas, split_k, upconv, post)
     if _conv_profiler is not None:
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         L.call("emo_conv_igemm", C.byref(d), _stream())
         e1.record()
-        # algorithmic flops of the convolution being computed; MMA passes actually issued per algorithmic product
-        # (sub-pixel mode issues 4 of the 9 taps)
-        _conv_profiler.rec.append((e0, e1, 2.0 * N * Do * Ho * Wo * w.cout * Ci * kd * kh * kw,
-                                   (6 if three else 3) * (4.0 / 9.0 if upconv else 1.0),
-                                   f"{N}x{Di}x{Hi}x{Wi}x{Ci}->{w.cout} k{kd}{kh}{kw} s{stride[1]} p{'h2' if a.f16 else (3 if three else 2)}"
-                                   + (" up2-subpixel" if upconv else "")))
+        _conv_profiler.rec.append((e0, e1) + prof)
     else:
         L.call("emo_conv_igemm", C.byref(d), _stream())
-    return out if post is None else post_ret
+    return ret
+
+
+def conv_plan(a: Split, w: PackedConvWeight, stride=(1, 1, 1), pad=None, bias=None, residual=None, res_shift: int = 0,
+              act: int = ACT_NONE, post_add=None, out_nchw: bool = False, stats: Optional[torch.Tensor] = None,
+              G: int = 32, out: Optional[torch.Tensor] = None, acc_chunk_mmas: int = 0, split_k: bool = True,
+              upconv: bool = False, post: Optional[dict] = None, sm_count: Optional[int] = None) -> L.ConvPlanInfo:
+    """The launch plan conv_igemm() would run for the same arguments on a device of `sm_count` SMs (default: the current
+    device's).  Nothing is launched; raises lib.EmoError where conv_igemm would refuse the arguments."""
+    d, _ret, _pd, _prof = _conv_desc(a, w, stride, pad, bias, residual, res_shift, act, post_add, out_nchw, stats, G, out,
+                                     acc_chunk_mmas, split_k, upconv, post)
+    if sm_count is None:
+        sm_count = torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
+    lib = L.load()
+    info = L.ConvPlanInfo()
+    rc = lib.emo_conv_plan(C.byref(d), int(sm_count), C.byref(info))
+    if rc != 0:
+        raise L.EmoError(f"emo_conv_plan failed ({rc}): {lib.emo_last_error().decode()}")
+    return info
 
 
 def conv_direct(x: torch.Tensor, w: torch.Tensor, stride: int, pad: int, bias=None, stats=None, G: int = 32):

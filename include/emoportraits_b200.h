@@ -35,7 +35,7 @@ extern "C" {
 enum { EMO_ACT_NONE = 0, EMO_ACT_RELU = 1, EMO_ACT_SIGMOID = 2, EMO_ACT_TANH = 3 };
 
 const char* emo_last_error(void);
-int emo_version(void); /* 104: + emo_composite; 103: emo_conv_desc.post; 102: + emo_u8_to_image, emo_image_to_u8, emo_resize_bicubic; 101: emo_pose_desc and emo_conv_desc gained trailing fields */
+int emo_version(void); /* 105: + emo_conv_plan; 104: + emo_composite; 103: emo_conv_desc.post; 102: + emo_u8_to_image, emo_image_to_u8, emo_resize_bicubic; 101: emo_pose_desc and emo_conv_desc gained trailing fields */
 /* sm count, and cc major*10+minor of the current device */
 int emo_device_info(int* sm_count, int* cc);
 
@@ -235,6 +235,40 @@ typedef struct {
   const struct emo_apply_desc_s* post;
 } emo_conv_desc;
 int emo_conv_igemm(const emo_conv_desc* d, void* stream);
+
+/* The launch plan emo_conv_igemm picks for a descriptor on a device with `sm_count` SMs.  Host arithmetic only: no CUDA
+ * call, no device needed, pointers are checked (null, alignment) but never dereferenced.  Runs the same argument checks
+ * and returns the same error codes as emo_conv_igemm. */
+enum {
+  EMO_CONV_KERNEL_BF16X2_KC64 = 0, /* conv_igemm_kernel<64, 2> */
+  EMO_CONV_KERNEL_BF16X2_KC32 = 1, /* conv_igemm_kernel<32, 2> */
+  EMO_CONV_KERNEL_BF16X3_KC64 = 2, /* conv_igemm_kernel<64, 3> */
+  EMO_CONV_KERNEL_BF16X3_KC32 = 3, /* conv_igemm_kernel<32, 3> */
+  EMO_CONV_KERNEL_F16_KC64 = 4,    /* conv_igemm_f16_kernel<64, 2> */
+  EMO_CONV_KERNEL_F16_KC32 = 5,    /* conv_igemm_f16_kernel<32, 2> */
+  EMO_CONV_KERNEL_UPCONV_KC64 = 6  /* conv_igemm_ps_kernel<64, 2> */
+};
+enum {
+  EMO_CONV_FINISH_NONE = 0,           /* the convolution kernel writes the output */
+  EMO_CONV_FINISH_FINALIZE = 1,       /* split-K: the finalize kernel sums the parts */
+  EMO_CONV_FINISH_POST = 2,           /* split-K with a post-op: one cluster kernel sums, normalises and writes the post-op */
+  EMO_CONV_FINISH_FINALIZE_APPLY = 3, /* split-K: finalize, then emo_apply runs the post-op */
+  EMO_CONV_FINISH_APPLY = 4           /* un-split with a post-op: emo_apply after the convolution kernel */
+};
+typedef struct {
+  int kernel;            /* EMO_CONV_KERNEL_* */
+  int KC, NP, fp16;      /* channels per k-chunk, operand planes, fp16 operands */
+  int BN;                /* N tile (output channels per tile) */
+  int ksplit;            /* K parts (1: not split) */
+  int yreuse, sa, sb;    /* row-reuse main loop, its A (halo tile) and B ring depths */
+  int stages;            /* pipeline stages (the B ring depth with row reuse) */
+  int flush;             /* k-steps per accumulation chunk */
+  int tw, th, td;        /* pixel box of one tile */
+  int m_tiles, n_tiles;  /* pixel tiles, N tiles (x4 output phases with upconv) */
+  int grid;              /* CTAs launched: min(m_tiles * n_tiles * ksplit, sm_count) */
+  int finish;            /* EMO_CONV_FINISH_* */
+} emo_conv_plan_info;
+int emo_conv_plan(const emo_conv_desc* d, int sm_count, emo_conv_plan_info* out);
 
 /* Direct fp32 SIMT convolution for the layers the tensor-core path does not take (Cin not a
  * multiple of 32: the RGB stems local_encoder.py:66-74 7x7 and torchvision resnet conv1).

@@ -10,7 +10,7 @@ ROOT = pathlib.Path(__file__).resolve().parents[1]
 PAIRS = {
     "GridSample3dDesc": "emo_grid_sample3d_desc", "GridSample2dAffineDesc": "emo_grid_sample2d_affine_desc",
     "ResizeBilinearDesc": "emo_resize_bilinear_desc", "GnFinalizeDesc": "emo_gn_finalize_desc", "ApplyDesc": "emo_apply_desc",
-    "GnHeadDesc": "emo_gn_head_desc", "ConvDesc": "emo_conv_desc", "ConvDirectDesc": "emo_conv_direct_desc",
+    "GnHeadDesc": "emo_gn_head_desc", "ConvDesc": "emo_conv_desc", "ConvPlanInfo": "emo_conv_plan_info", "ConvDirectDesc": "emo_conv_direct_desc",
     "LinearDesc": "emo_linear_desc", "ResampleDesc": "emo_resample_desc", "PoseDesc": "emo_pose_desc",
 }
 
@@ -19,7 +19,7 @@ def _c_name(f):
     return f[:-1] if f.endswith("_") and f[:-1] in ("in",) else f
 
 
-def test_ctypes_structures_match_the_header(tmp_path):
+def test_every_ctypes_structure_matches_the_header(tmp_path):
     from emoportraits_b200 import lib as L
 
     structs = {n: getattr(L, n) for n in PAIRS}

@@ -58,7 +58,8 @@ def _check(case, img, so, name):
 def test_upconv_subpixel_matches_conv_on_upsampled_planes(Cin, Cout, S, residual):
     """conv_igemm(low-res planes, folded weights, upconv=True) == conv_igemm(nearest-x2 planes, 3x3 weights): same operands
     up to the fp32 pre-summing of the folded taps, so agreement to ~2^-15 of the output scale; statistics likewise.
-    S = 256 (-> 512^2, 2048 tiles) takes the store-warp (EPI = 1) variant of the kernel, the others EPI = 0."""
+    At 132 SMs the cases plan ps<64,2> with BN 128 (row reuse, 2 halo tiles; S = 256 gives 4096 work items), BN 32 and BN 80
+    (3 halo tiles); tests/test_conv_plan_gpu.py sweeps every plan class of this kernel."""
     import math
 
     from emoportraits_b200 import ops

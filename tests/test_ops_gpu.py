@@ -192,9 +192,9 @@ def test_conv_igemm_three_planes(ops, Cin, Cout, sp, k):
 
 
 @pytest.mark.parametrize("N,Cin,Cout,sp,k,planes,kw", [
-    (1, 64, 96, (24, 40), 3, 2, dict(residual=True, stats=True)),          # ragged pixel tiles: TMA clips the store, zero-fills the residual
-    (1, 64, 128, (256, 256), 3, 2, dict(residual=False, stats=True)),      # no residual, several tiles per CTA: staging tile written directly
-    (1, 512, 320, (32, 32), 3, 2, dict(residual=True, stats=True)),        # N tile 160: five panels
+    (1, 64, 96, (24, 40), 3, 2, dict(residual=True, stats=True)),          # ragged pixel boxes: conv<64,2> BN16 rr3, per-column statistics
+    (1, 64, 128, (256, 256), 3, 2, dict(residual=False, stats=True)),      # no residual, several tiles per CTA: conv<64,2> BN128 rr2
+    (1, 512, 320, (32, 32), 3, 2, dict(residual=True, stats=True)),        # 20 N tiles of 16 (BN narrowed from 80 on 8 pixel tiles)
     (2, 64, 96, (16, 32), 3, 2, dict(residual=True, stats=True, act=3)),   # batch of 2 (per-sample statistics), tanh
     (1, 64, 128, (32, 32), 3, 2, dict(residual=True, res_shift=1, stats=True)),  # half-resolution residual: quarter-size TMA tile
     (1, 64, 128, (24, 40), 3, 2, dict(residual=True, res_shift=1, stats=True)),  # the same on ragged tiles
