@@ -102,6 +102,12 @@ __device__ __forceinline__ void split_f16(float x, __half& hi, __half& lo) {
   hi = __float2half_rn(x);
   lo = __float2half_rn(x - __half2float(hi));
 }
+// One-plane fp16 operand mode (emo_conv_desc.operand_fp16 with a_lo == w_lo == NULL): the plane is the hi plane of the split
+// above, fp16(x * s) with the same saturation; one fp16 MMA per product, ~2^-11 relative per operand.
+__device__ __forceinline__ __half f16_plane(float xs) { return __float2half_rn(fminf(fmaxf(xs, -65000.f), 65000.f)); }
+__device__ __forceinline__ uint2 plane4_h(const float4& v, float s) {
+  return make_uint2(pack_f16x2(f16_plane(v.x * s), f16_plane(v.y * s)), pack_f16x2(f16_plane(v.z * s), f16_plane(v.w * s)));
+}
 __device__ __forceinline__ void split4_h(const float4& v, float s, uint2& hi, uint2& lo) {
   __half h0, h1, h2, h3, l0, l1, l2, l3;
   split_f16(v.x * s, h0, l0);

@@ -15,7 +15,8 @@
 //   hi*hi + hi*lo + lo*hi (3 wgmmas per 16 channels; 6 products with three planes) into an fp32 register accumulator.
 //   The tensor core accumulates with truncation, so an accumulator only takes a short chunk of MMAs (24 / 48); every chunk
 //   is then added to a second set of fp32 registers with round-to-nearest adds.  Plain bf16/tf32 operands, or one long
-//   accumulation chain, do not hold the 1e-3 budget.
+//   accumulation chain, do not hold the 1e-3 budget.  The decoder's opt-in fast mode takes ONE scaled fp16 plane per operand
+//   (a_lo == w_lo == NULL): one wgmma per product, ~2^-11 relative per operand (DESIGN.md section 2).
 // Warp roles: warps 0..7 = two consumer warpgroups (64 tile rows each: wgmma issue, chunk promotion, final phase),
 //   warps 8..11 = producer warpgroup (warp 8: TMA, one elected lane issues).
 // Main loop: stride-1 convolutions load ONE halo A tile per (kernel column, k-chunk) and serve its kh tap rows through
@@ -211,6 +212,11 @@ struct TMaps {
 #define EMO_CONV_KERNEL_NAME conv_igemm_f16_kernel
 #include "conv_igemm_kernel.inc"
 #undef EMO_CONV_PS
+#undef EMO_CONV_KERNEL_NAME
+#define EMO_CONV_PS 1
+#define EMO_CONV_KERNEL_NAME conv_igemm_ps_f16_kernel
+#include "conv_igemm_kernel.inc"
+#undef EMO_CONV_PS
 #undef EMO_CONV_F16
 #undef EMO_CONV_KERNEL_NAME
 
@@ -404,7 +410,9 @@ __global__ void __launch_bounds__(kPostThreads, 1) splitk_post_kernel(const Post
       y = act_apply(y, a.act);
       if (a.out) a.out[i] = y;
       if (a.out_hi) {
-        if (a.plane_fp16) {
+        if (a.plane_fp16 && !a.out_lo) {
+          ((__half*)a.out_hi)[i] = f16_plane(y * a.plane_scale);
+        } else if (a.plane_fp16) {
           __half h, l;
           split_f16(y * a.plane_scale, h, l);
           ((__half*)a.out_hi)[i] = h; ((__half*)a.out_lo)[i] = l;
@@ -460,7 +468,12 @@ static int plan_conv(const emo_conv_desc* d, int sm_count, ConvPlan* plan) {
   EMO_REQUIRE(plan && sm_count >= 1, "emo_conv_igemm: bad plan arguments (sm_count=%d)", sm_count);
   memset(plan, 0, sizeof(*plan));
   ConvKParams& p = plan->p;
-  EMO_REQUIRE(d && d->a_hi && d->a_lo && d->w_hi && d->w_lo && d->out, "emo_conv_igemm: null pointer");
+  // one-plane fp16 operands: a_lo == w_lo == NULL with operand_fp16 (a_lo2 / w_lo2 then must be NULL too)
+  const bool one_plane = d && !d->a_lo && !d->w_lo;
+  EMO_REQUIRE(d && d->a_hi && d->w_hi && d->out && (one_plane || (d->a_lo && d->w_lo)),
+              "emo_conv_igemm: null pointer (a_lo and w_lo are both given, or both NULL for one-plane fp16 operands)");
+  EMO_REQUIRE(!one_plane || (d->operand_fp16 && !d->a_lo2 && !d->w_lo2),
+              "emo_conv_igemm: one-plane operands (a_lo == w_lo == NULL) are fp16 only (operand_fp16) and take no a_lo2 / w_lo2");
   EMO_REQUIRE(d->Cin % 32 == 0, "emo_conv_igemm: Cin=%d must be a multiple of 32 (use emo_conv_direct)", d->Cin);
   EMO_REQUIRE(d->Cout_pad % 16 == 0 && d->Cout <= d->Cout_pad, "emo_conv_igemm: Cout_pad=%d must be a multiple of 16 >= Cout", d->Cout_pad);
   EMO_REQUIRE(d->sd >= 1 && d->sh >= 1 && d->sw >= 1 && d->sd <= 2 && d->sh <= 2 && d->sw <= 2, "emo_conv_igemm: stride must be 1 or 2");
@@ -476,7 +489,7 @@ static int plan_conv(const emo_conv_desc* d, int sm_count, ConvPlan* plan) {
   const bool vec_ok = (d->Cout % 4 == 0);
   EMO_REQUIRE(vec_ok || d->Cout < 16, "emo_conv_igemm: Cout=%d must be a multiple of 4 (or < 16)", d->Cout);
 
-  const int NP = d->a_lo2 ? 3 : 2;
+  const int NP = one_plane ? 1 : d->a_lo2 ? 3 : 2;
   EMO_REQUIRE((d->a_lo2 == nullptr) == (d->w_lo2 == nullptr), "emo_conv_igemm: a_lo2 and w_lo2 must be given together");
   // sub-pixel mode: the descriptor describes conv3x3(pad 1)(nearest_x2(input)) with the input given at LOW resolution and
   // the weights pre-folded to [4 phases][2x2 taps][Cout_pad][Cin] (emoportraits_b200/ops.py: pack_upconv_weight)
@@ -486,11 +499,12 @@ static int plan_conv(const emo_conv_desc* d, int sm_count, ConvPlan* plan) {
                 "emo_conv_igemm: upconv needs a 1x3x3 stride-1 pad-1 convolution");
     EMO_REQUIRE(d->Din == 1 && d->Dout == 1 && d->Hout == 2 * d->Hin && d->Wout == 2 * d->Win,
                 "emo_conv_igemm: upconv output must be (2 Hin, 2 Win) (got %d x %d from %d x %d)", d->Hout, d->Wout, d->Hin, d->Win);
-    EMO_REQUIRE(NP == 2 && d->Cin % 64 == 0 && d->Cout == d->Cout_pad && !d->out_nchw,
-                "emo_conv_igemm: upconv needs two-plane operands, Cin %% 64 == 0, Cout %% 16 == 0, channels-last output");
+    EMO_REQUIRE(NP <= 2 && d->Cin % 64 == 0 && d->Cout == d->Cout_pad && !d->out_nchw,
+                "emo_conv_igemm: upconv needs two-plane bf16 or one-plane fp16 operands, Cin %% 64 == 0, Cout %% 16 == 0, channels-last output");
   }
   const int f16 = d->operand_fp16 ? 1 : 0;
-  if (f16) EMO_REQUIRE(NP == 2 && !ps && d->out_scale > 0.f, "emo_conv_igemm: fp16 operands need two planes, no upconv, out_scale > 0");
+  if (f16) EMO_REQUIRE(NP <= 2 && !(ps && NP == 2) && d->out_scale > 0.f,
+                       "emo_conv_igemm: fp16 operands need one or two planes (upconv: one), out_scale > 0");
   const int gH = ps ? d->Hin : d->Hout, gW = ps ? d->Win : d->Wout;  // the pixel grid the tiles walk
   const int taps_k = ps ? 4 : d->kd * d->kh * d->kw;                  // taps in one tile's K loop
   const int nt_mult = ps ? 4 : 1;                                     // N tiles per channel tile (one per output phase)
@@ -597,9 +611,11 @@ static int plan_conv(const emo_conv_desc* d, int sm_count, ConvPlan* plan) {
   EMO_REQUIRE(!ps || KC == 64, "emo_conv_igemm: upconv tile does not fit with KC = 64");
   p.stages = stages;
   {
-    // ~24 MMAs per accumulation chunk keeps the truncation bias of the tensor-core accumulator near 1e-6 relative
-    const int mmas_per_kstep = (KC / 16) * (NP == 3 ? 6 : 3);
-    const int target = d->acc_chunk_mmas > 0 ? d->acc_chunk_mmas : (NP == 3 ? 24 : 48);
+    // ~24 MMAs per accumulation chunk keeps the truncation bias of the tensor-core accumulator near 1e-6 relative; one-plane
+    // operands: 16 MMAs = 256 channels of K (every MMA adds a full-size term: measured on an H100, 32 MMAs leave a bias of
+    // -2.6e-6 relative, tests/test_fast_decoder_gpu.py)
+    const int mmas_per_kstep = (KC / 16) * (NP == 3 ? 6 : NP == 2 ? 3 : 1);
+    const int target = d->acc_chunk_mmas > 0 ? d->acc_chunk_mmas : (NP == 3 ? 24 : NP == 2 ? 48 : 16);
     p.flush = target / mmas_per_kstep < 1 ? 1 : target / mmas_per_kstep;
   }
   const size_t smem_bytes = ring_bytes + tail_bytes + 1024;
@@ -615,7 +631,8 @@ static int plan_conv(const emo_conv_desc* d, int sm_count, ConvPlan* plan) {
   else
     plan->finish = post ? EMO_CONV_FINISH_APPLY : EMO_CONV_FINISH_NONE;
   plan->NP = NP; plan->KC = KC; plan->f16 = f16; plan->ps = ps; plan->kh_eff = kh_eff;
-  plan->kernel = f16 ? (KC == 64 ? EMO_CONV_KERNEL_F16_KC64 : EMO_CONV_KERNEL_F16_KC32)
+  plan->kernel = NP == 1 ? (ps ? EMO_CONV_KERNEL_H1_UPCONV_KC64 : KC == 64 ? EMO_CONV_KERNEL_H1_KC64 : EMO_CONV_KERNEL_H1_KC32)
+                 : f16 ? (KC == 64 ? EMO_CONV_KERNEL_F16_KC64 : EMO_CONV_KERNEL_F16_KC32)
                  : ps ? EMO_CONV_KERNEL_UPCONV_KC64
                  : NP == 3 ? (KC == 64 ? EMO_CONV_KERNEL_BF16X3_KC64 : EMO_CONV_KERNEL_BF16X3_KC32)
                            : (KC == 64 ? EMO_CONV_KERNEL_BF16X2_KC64 : EMO_CONV_KERNEL_BF16X2_KC32);
@@ -714,7 +731,11 @@ extern "C" int emo_conv_igemm(const emo_conv_desc* d, void* stream_) {
     e = cudaGetLastError();                                                                                               \
     if (e != cudaSuccess) { set_error("emo_conv_igemm: launch: %s", cudaGetErrorString(e)); return EMO_ERR_CUDA; }         \
   } while (0)
-  if (f16) {
+  if (NP == 1) {
+    if (ps) EMO_LAUNCH_CONV(conv_igemm_ps_f16_kernel, 64, 1);
+    else if (KC == 64) EMO_LAUNCH_CONV(conv_igemm_f16_kernel, 64, 1);
+    else EMO_LAUNCH_CONV(conv_igemm_f16_kernel, 32, 1);
+  } else if (f16) {
     if (KC == 64) EMO_LAUNCH_CONV(conv_igemm_f16_kernel, 64, 2);
     else EMO_LAUNCH_CONV(conv_igemm_f16_kernel, 32, 2);
   } else if (ps) {

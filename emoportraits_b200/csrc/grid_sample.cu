@@ -25,6 +25,8 @@ struct GS3Params {
   __nv_bfloat16* out_lo;
   __nv_bfloat16* out_lo2;
   long long os_n, os_c, os_d, os_h, os_w;
+  int plane_fp16;     // one fp16 plane of y * plane_scale in out_hi (out_lo / out_lo2 NULL)
+  float plane_scale;
   // brick decomposition of the output lattice (channels-last kernel)
   int bw, bh, bd, bricks_w, bricks_h, bricks_d;
 };
@@ -167,21 +169,27 @@ __global__ void __launch_bounds__(256) gs3_cl_kernel(const GS3Params p) {
       if (p.out) stg_hint((float4*)(p.out + o), acc, pol_out);  // the output is not re-read by this kernel
       if (SPLIT) {
         uint2 hi, lo, lo2;
-        if (p.out_lo2) {
-          split4x3(acc, hi, lo, lo2);
-          *(uint2*)(p.out_lo2 + o) = lo2;
+        if (p.plane_fp16) {
+          *(uint2*)(p.out_hi + o) = plane4_h(acc, p.plane_scale);
         } else {
-          split4(acc, hi, lo);
+          if (p.out_lo2) {
+            split4x3(acc, hi, lo, lo2);
+            *(uint2*)(p.out_lo2 + o) = lo2;
+          } else {
+            split4(acc, hi, lo);
+          }
+          *(uint2*)(p.out_hi + o) = hi;
+          *(uint2*)(p.out_lo + o) = lo;
         }
-        *(uint2*)(p.out_hi + o) = hi;
-        *(uint2*)(p.out_lo + o) = lo;
       }
     } else {
       const float a[4] = {acc.x, acc.y, acc.z, acc.w};
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         if (p.out) p.out[o + j * p.os_c] = a[j];
-        if (SPLIT) {
+        if (SPLIT && p.plane_fp16) {
+          ((__half*)p.out_hi)[o + j * p.os_c] = f16_plane(a[j] * p.plane_scale);
+        } else if (SPLIT) {
           __nv_bfloat16 h, l, l2;
           split_bf16x3(a[j], h, l, l2);
           if (!p.out_lo2) split_bf16(a[j], h, l);
@@ -311,14 +319,18 @@ __global__ void __launch_bounds__(1024, 1) gs3_bulk_kernel(const GS3Params p) {
         if (p.out) stg_hint((float4*)(p.out + o), acc, pol_out);
         if (SPLIT) {
           uint2 hi, lo, lo2;
-          if (p.out_lo2) {
-            split4x3(acc, hi, lo, lo2);
-            *(uint2*)(p.out_lo2 + o) = lo2;
+          if (p.plane_fp16) {
+            *(uint2*)(p.out_hi + o) = plane4_h(acc, p.plane_scale);
           } else {
-            split4(acc, hi, lo);
+            if (p.out_lo2) {
+              split4x3(acc, hi, lo, lo2);
+              *(uint2*)(p.out_lo2 + o) = lo2;
+            } else {
+              split4(acc, hi, lo);
+            }
+            *(uint2*)(p.out_hi + o) = hi;
+            *(uint2*)(p.out_lo + o) = lo;
           }
-          *(uint2*)(p.out_hi + o) = hi;
-          *(uint2*)(p.out_lo + o) = lo;
         }
       }
       __syncwarp();
@@ -361,7 +373,9 @@ __global__ void __launch_bounds__(256) gs3_nc_kernel(const GS3Params p) {
 #pragma unroll
       for (int j = 0; j < 8; ++j) acc = fmaf(__ldg(s + off[j]), wgt[j], acc);
       if (p.out) p.out[o + (long long)c * p.os_c] = acc;
-      if (p.out_hi) {
+      if (p.out_hi && p.plane_fp16) {
+        ((__half*)p.out_hi)[o + (long long)c * p.os_c] = f16_plane(acc * p.plane_scale);
+      } else if (p.out_hi) {
         __nv_bfloat16 h, l, l2;
         split_bf16x3(acc, h, l, l2);
         if (!p.out_lo2) split_bf16(acc, h, l);
@@ -564,7 +578,12 @@ extern "C" int emo_grid_sample3d(const emo_grid_sample3d_desc* d, void* stream_)
   cudaStream_t stream = (cudaStream_t)stream_;
   EMO_REQUIRE(d && d->in, "emo_grid_sample3d: null input");
   EMO_REQUIRE((d->grid != nullptr) != (d->theta != nullptr), "emo_grid_sample3d: exactly one of grid/theta must be given");
-  EMO_REQUIRE(d->out || (d->out_hi && d->out_lo), "emo_grid_sample3d: no output");
+  EMO_REQUIRE(d->out || (d->out_hi && (d->out_lo || d->plane_fp16)), "emo_grid_sample3d: no output");
+  EMO_REQUIRE((!d->out_lo || d->out_hi) && (!d->out_hi || d->out_lo || d->plane_fp16) && (!d->out_lo2 || d->out_lo),
+              "emo_grid_sample3d: operand planes are out_hi + out_lo [+ out_lo2], or out_hi alone with plane_fp16");
+  if (d->out_hi && d->plane_fp16)
+    EMO_REQUIRE(!d->out_lo && !d->out_lo2 && d->plane_scale > 0.f,
+                "emo_grid_sample3d: plane_fp16 writes one plane (out_lo, out_lo2 NULL) and needs plane_scale > 0");
   EMO_REQUIRE(d->N > 0 && d->C > 0 && d->Din > 0 && d->Hin > 0 && d->Win > 0 && d->Dout > 0 && d->Hout > 0 && d->Wout > 0,
               "emo_grid_sample3d: bad shape");
   GS3Params p;
@@ -574,6 +593,7 @@ extern "C" int emo_grid_sample3d(const emo_grid_sample3d_desc* d, void* stream_)
   p.out = d->out; p.out_hi = (__nv_bfloat16*)d->out_hi; p.out_lo = (__nv_bfloat16*)d->out_lo;
   p.out_lo2 = (__nv_bfloat16*)d->out_lo2;
   p.os_n = d->os_n; p.os_c = d->os_c; p.os_d = d->os_d; p.os_h = d->os_h; p.os_w = d->os_w;
+  p.plane_fp16 = d->out_hi ? d->plane_fp16 : 0; p.plane_scale = d->plane_scale;
   if (d->in_layout == 1) {
     EMO_REQUIRE(d->C % 4 == 0, "emo_grid_sample3d: channels-last path needs C %% 4 == 0 (C=%d)", d->C);
     EMO_REQUIRE(((uintptr_t)d->in % 16) == 0, "emo_grid_sample3d: input must be 16-byte aligned");

@@ -177,9 +177,14 @@ __global__ void split_kernel(const float* __restrict__ x, long long n4, uint2* _
 
 __global__ void split_f16_kernel(const float* __restrict__ x, long long n4, float scale, uint2* __restrict__ hi, uint2* __restrict__ lo) {
   for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < n4; t += (long long)gridDim.x * blockDim.x) {
-    uint2 h, l;
-    split4_h(__ldg((const float4*)x + t), scale, h, l);
-    hi[t] = h; lo[t] = l;
+    const float4 v = __ldg((const float4*)x + t);
+    if (lo) {
+      uint2 h, l;
+      split4_h(v, scale, h, l);
+      hi[t] = h; lo[t] = l;
+    } else {
+      hi[t] = plane4_h(v, scale);
+    }
   }
 }
 
@@ -229,7 +234,9 @@ extern "C" int emo_gn_finalize(const emo_gn_finalize_desc* d, void* stream_) {
 extern "C" int emo_apply(const emo_apply_desc* d, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   EMO_REQUIRE(d && d->x, "emo_apply: null input");
-  EMO_REQUIRE(d->out || (d->out_hi && d->out_lo), "emo_apply: no output");
+  EMO_REQUIRE(d->out || (d->out_hi && (d->out_lo || d->plane_fp16)), "emo_apply: no output");
+  EMO_REQUIRE((!d->out_lo || d->out_hi) && (!d->out_hi || d->out_lo || d->plane_fp16),
+              "emo_apply: operand planes are out_hi + out_lo, or out_hi alone with plane_fp16");
   EMO_REQUIRE(d->C % 4 == 0, "emo_apply: C=%d must be a multiple of 4", d->C);
   EMO_REQUIRE(d->up == 1 || d->up == 2, "emo_apply: up must be 1 or 2");
   EMO_REQUIRE((d->A == nullptr) == (d->B == nullptr) && (d->A2 == nullptr) == (d->B2 == nullptr), "emo_apply: A/B must come in pairs");
@@ -246,7 +253,7 @@ extern "C" int emo_apply(const emo_apply_desc* d, void* stream_) {
   const size_t smem = d->stats ? 2 * (size_t)d->C * sizeof(float) : 0;
   EMO_REQUIRE(smem <= 48 * 1024, "emo_apply: C=%d too large for the fused finalisation", d->C);
   if (d->plane_fp16) {
-    EMO_REQUIRE(!d->out_lo2 && d->plane_scale > 0.f, "emo_apply: fp16 planes come in pairs and need a positive plane_scale");
+    EMO_REQUIRE(!d->out_lo2 && d->plane_scale > 0.f, "emo_apply: fp16 planes are one or two (no out_lo2) and need a positive plane_scale");
     if (d->up == 1 && V == 2) launch_kernel(apply_f16_kernel<1, 2>, grid, 256, smem, stream, *d);
     else if (d->up == 1) launch_kernel(apply_f16_kernel<1, 1>, grid, 256, smem, stream, *d);
     else if (V == 2) launch_kernel(apply_f16_kernel<2, 2>, grid, 256, smem, stream, *d);
@@ -289,7 +296,7 @@ extern "C" int emo_split_bf16(const float* x, long long n, void* hi, void* lo, v
 
 extern "C" int emo_split_f16(const float* x, long long n, float scale, void* hi, void* lo, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
-  EMO_REQUIRE(x && hi && lo, "emo_split_f16: null pointer");
+  EMO_REQUIRE(x && hi, "emo_split_f16: null pointer");
   EMO_REQUIRE(n % 4 == 0 && scale > 0.f, "emo_split_f16: n must be a multiple of 4 and scale positive");
   long long blocks = cdivll(n / 4, 256);
   if (blocks > 132ll * 32) blocks = 132ll * 32;

@@ -32,18 +32,39 @@ class Model:
     # ~2^-22 relative, i.e. fp32-faithful — for the embedding / warp networks, whose output the sampler differentiates (an
     # error of 1e-4 in the embedding moves the image by 1e-2), and for the source-pass networks.  Three bf16 planes (6 MMAs,
     # the round-1 setting of those networks) give the same accuracy at twice the MMAs (tests/test_conv_modes_gpu.py) and
-    # remain available through `precision=`.  The decoder's input planes are written by grid_sample_3d in bf16.
+    # remain available through `precision=`.  The decoder's input planes are written by grid_sample_3d in bf16 (or, with
+    # decoder=ops.H1, as one fp16 plane).
     PRECISION = dict(head_pose=ops.H2, expression=ops.H2, idt=ops.H2, warp=ops.H2, local_encoder=ops.H2, volume_source=ops.H2,
                      unet3d=ops.H2, decoder=2)
+    # Named settings of `precision=`: "exact" is PRECISION; "fast" runs the decoder on one fp16 plane (ops.H1: one MMA per
+    # product instead of three).  Fast mode keeps every uint8 output pixel within one level of the exact path
+    # (tools/decoder_precision_emulation.py, tests/test_fast_decoder_gpu.py; INTEGRATION.md "Fast mode").
+    PRESETS = dict(exact={}, fast=dict(decoder=ops.H1))
 
-    def __init__(self, cfg: HotPathConfig, state_dict, head_pose_state_dict, device="cuda", precision: Optional[dict] = None):
+    @classmethod
+    def resolve_precision(cls, precision) -> dict:
+        """`precision=` of Model: None, a preset name ("exact" / "fast") or a dict of per-network overrides of PRECISION"""
+        if precision is None or isinstance(precision, str):
+            if (precision or "exact") not in cls.PRESETS:
+                raise ValueError(f"precision={precision!r}: the named settings are {sorted(cls.PRESETS)}")
+            precision = cls.PRESETS[precision or "exact"]
+        pr = dict(cls.PRECISION)
+        pr.update(precision)
+        if pr["decoder"] == ops.H2:
+            raise ValueError("the decoder's input planes are written by grid_sample_3d in bf16 or as one fp16 plane; it runs "
+                             "with 2 or 3 bf16 planes or ops.H1")
+        one_plane = sorted(net for net, planes in pr.items() if planes == ops.H1 and net != "decoder")
+        if one_plane:
+            raise ValueError(f"ops.H1 (one fp16 plane) is for the decoder only, not {one_plane}: the embedding and warp networks "
+                             "feed the sampler, which amplifies their errors ~100x (DESIGN.md section 2)")
+        return pr
+
+    def __init__(self, cfg: HotPathConfig, state_dict, head_pose_state_dict, device="cuda", precision=None):
+        """precision: None / "exact" (PRECISION), "fast" (decoder on ops.H1), or a dict overriding PRECISION per network."""
         self.cfg = cfg
         dev = torch.device(device)
         sd = state_dict
-        pr = dict(self.PRECISION)
-        pr.update(precision or {})
-        if pr["decoder"] == ops.H2:
-            raise ValueError("the decoder's input planes are written by grid_sample_3d in bf16; it runs with 2 or 3 bf16 planes")
+        pr = self.resolve_precision(precision)
         self.precision = pr
         self.local_encoder_nw = nets.LocalEncoder(sd, cfg, dev, planes=pr["local_encoder"])
         self.idt_embedder_nw = nets.IdtEmbed(sd, cfg, dev, planes=pr["idt"])
@@ -250,8 +271,13 @@ class InferenceWrapper(torch.nn.Module):
     def __init__(self, experiment_name, which_epoch='latest', model_file_name='', use_gpu=True, num_gpus=1,
                  fixed_bounding_box=False, project_dir='./', folder='mp_logs', model_='va',
                  torch_home='', debug=False, print_model=False, print_params=True, args_overwrite={}, state_dict=None,
-                 pose_momentum=0.5, rank=0, args_path=None, head_pose_state_dict=None):
+                 pose_momentum=0.5, rank=0, args_path=None, head_pose_state_dict=None, precision="exact"):
+        """precision: "exact" (default: the parity path) or "fast" (the decoder on one fp16 plane: every uint8 output pixel
+        within one level of "exact", INTEGRATION.md "Fast mode").  Every driver path (captured pipelines, the list form of
+        forward, video.drive_image_with_video) runs with the model's setting."""
         super().__init__()
+        if precision not in ("exact", "fast"):
+            raise ValueError(f"precision={precision!r}: 'exact' or 'fast'")
         if not use_gpu or not torch.cuda.is_available():
             raise RuntimeError("emoportraits_b200.InferenceWrapper needs a CUDA device (H100); there is no CPU path")
         if model_ != 'va':
@@ -274,7 +300,8 @@ class InferenceWrapper(torch.nn.Module):
             if not hp or not pathlib.Path(str(hp)).exists():
                 raise FileNotFoundError(f"head pose regressor checkpoint not found ({hp}); pass head_pose_state_dict=")
             head_pose_state_dict = torch.load(hp, map_location='cpu')
-        self.model = Model(self.cfg, state_dict, head_pose_state_dict, self.device)
+        self.precision = precision
+        self.model = Model(self.cfg, state_dict, head_pose_state_dict, self.device, precision=precision)
         if rank == 0 and print_params:
             n = sum(v.numel() for v in state_dict.values())
             print(f'Number of parameters/buffers in checkpoint: {n}')

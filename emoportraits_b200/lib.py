@@ -22,7 +22,8 @@ class GridSample3dDesc(C.Structure):
     _fields_ = [("in_", c_void_p), ("in_layout", c_int), ("N", c_int), ("C", c_int), ("Din", c_int), ("Hin", c_int),
                 ("Win", c_int), ("grid", c_void_p), ("theta", c_void_p), ("Dout", c_int), ("Hout", c_int),
                 ("Wout", c_int), ("out", c_void_p), ("out_hi", c_void_p), ("out_lo", c_void_p), ("os_n", c_ll),
-                ("os_c", c_ll), ("os_d", c_ll), ("os_h", c_ll), ("os_w", c_ll), ("out_lo2", c_void_p)]
+                ("os_c", c_ll), ("os_d", c_ll), ("os_h", c_ll), ("os_w", c_ll), ("out_lo2", c_void_p),
+                ("plane_fp16", c_int), ("plane_scale", c_float)]
 
 
 class GridSample2dAffineDesc(C.Structure):
@@ -78,6 +79,13 @@ class ConvPlanInfo(C.Structure):
 # emo_conv_plan_info.kernel and .finish (EMO_CONV_KERNEL_* / EMO_CONV_FINISH_*)
 CONV_KERNELS = ("conv<64,2>", "conv<32,2>", "conv<64,3>", "conv<32,3>", "f16<64,2>", "f16<32,2>", "ps<64,2>")
 CONV_FINISH = ("none", "finalize", "post", "finalize+apply", "apply")
+# the one-plane fp16 kernels (operand mode ops.H1) follow as ids 7, 8, 9 (EMO_CONV_KERNEL_H1_*)
+CONV_KERNELS_H1 = ("h1<64,1>", "h1<32,1>", "h1ps<64,1>")
+
+
+def conv_kernel_name(kernel: int) -> str:
+    """name of an emo_conv_plan_info.kernel id"""
+    return (CONV_KERNELS + CONV_KERNELS_H1)[kernel]
 
 
 class ConvDirectDesc(C.Structure):

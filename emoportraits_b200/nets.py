@@ -76,11 +76,12 @@ class ResBlock:
         # sub-pixel form of `nearest x2 -> norm -> relu -> 3x3 conv` for blocks called with up=2 (ops.pack_upconv_weight):
         # the conv then reads the LOW-resolution planes (4/9 of the MMAs, no upsampled operand; measured round 2: 229 -> 244
         # frames/s).  Shapes the sub-pixel kernel does not take (Cout % 32, Cin % 64, odd pixel-tile count) use the plain form.
+        # Two bf16 planes or one fp16 plane (ops.H1).
         self.c1_ps = None
-        if subpixel_up and planes == 2:
+        if subpixel_up and planes in (2, ops.H1):
             w, _ = fold_conv(sd, p + ".block_feats.2", ws=ws_first)
             if tuple(w.shape[2:]) == (3, 3) and w.shape[0] % 32 == 0 and w.shape[1] % 64 == 0:
-                self.c1_ps = ops.pack_upconv_weight(w, device=dev)
+                self.c1_ps = ops.pack_upconv_weight(w, device=dev, planes=planes)
         self.n2 = Norm(sd, p + ".block_feats.3", dev)
         self.c2 = ConvW(sd, p + ".block.0", dev, planes=planes)
         self.skip = ConvW(sd, p + ".skip.0", dev, planes=planes) if (p + ".skip.0.weight_orig") in sd else None

@@ -41,6 +41,10 @@ def _chk(t: torch.Tensor, dtype=torch.float32):
 H2 = "h2"
 F16_ACT_SCALE = 16.0    # activations: post-GroupNorm / ReLU values are O(1)
 F16_W_SCALE = 256.0     # spectral-norm / weight-standardised weights are O(0.01 .. 1)
+# fp16 one-plane operand mode ("h1"): ONE fp16 plane of (value * the same power of two as "h2"), one MMA per product instead of
+# three, ~2^-11 relative per operand.  Decoder only (DESIGN.md section 2): the embedding / warp networks feed the sampler, which
+# amplifies their errors ~100x (tools/decoder_precision_emulation.py gives the decoder's bounds).
+H1 = "h1"
 
 
 # MMAs per accumulation chunk (the tensor core accumulates with truncation: DESIGN.md section 2).  bf16 two-plane operands
@@ -54,15 +58,16 @@ ACC_CHUNK_F16 = 24
 
 
 def _nplanes(planes) -> int:
-    return 2 if planes == H2 else int(planes)
+    return 2 if planes == H2 else 1 if planes == H1 else int(planes)
 
 
 @dataclass
 class Split:
     """operand planes of a channels-last activation (N, D, H, W, C): bf16 (hi, lo) — or (hi, lo, lo2) in the fp32-faithful
-    three-plane mode used by the numerically sensitive networks — or, with f16 = True, fp16 (hi, lo) of value * scale."""
+    three-plane mode used by the numerically sensitive networks — or, with f16 = True, fp16 (hi, lo) of value * scale, or
+    fp16 hi alone (lo None: the one-plane mode H1)."""
     hi: torch.Tensor
-    lo: torch.Tensor
+    lo: Optional[torch.Tensor]
     lo2: Optional[torch.Tensor] = None
     f16: bool = False
     scale: float = 1.0
@@ -73,10 +78,12 @@ class Split:
 
     @property
     def planes(self) -> int:
-        return 3 if self.lo2 is not None else 2
+        return 3 if self.lo2 is not None else 2 if self.lo is not None else 1
 
     @staticmethod
     def empty(shape, device, planes=2) -> "Split":
+        if planes == H1:
+            return Split(torch.empty(tuple(shape), dtype=torch.float16, device=device), None, None, True, F16_ACT_SCALE)
         if planes == H2:
             buf = torch.empty((2,) + tuple(shape), dtype=torch.float16, device=device)
             return Split(buf[0], buf[1], None, True, F16_ACT_SCALE)
@@ -84,37 +91,39 @@ class Split:
         return Split(buf[0], buf[1], buf[2] if planes == 3 else None)
 
     def view(self, *shape) -> "Split":
-        return Split(self.hi.view(*shape), self.lo.view(*shape), self.lo2.view(*shape) if self.lo2 is not None else None,
-                     self.f16, self.scale)
+        return Split(self.hi.view(*shape), self.lo.view(*shape) if self.lo is not None else None,
+                     self.lo2.view(*shape) if self.lo2 is not None else None, self.f16, self.scale)
 
     def float(self) -> torch.Tensor:
-        f = self.hi.float() + self.lo.float()
+        f = self.hi.float() + self.lo.float() if self.lo is not None else self.hi.float()
         f = f + self.lo2.float() if self.lo2 is not None else f
         return f / self.scale if self.f16 else f
 
 
 @dataclass
 class PackedConvWeight:
-    """Conv weight in the kernel-native layout: bf16 planes [taps][Cout_pad][Cin] (taps = kd*kh*kw)."""
+    """Conv weight in the kernel-native layout: bf16 planes [taps][Cout_pad][Cin] (taps = kd*kh*kw); fp16 planes of
+    weight * scale with f16 (lo None: the one-plane mode H1)."""
     hi: torch.Tensor
-    lo: torch.Tensor
+    lo: Optional[torch.Tensor]
     cout: int
     cout_pad: int
     cin: int
     k: tuple  # (kd, kh, kw)
     lo2: Optional[torch.Tensor] = None
-    acc_chunk: int = 0  # MMAs per accumulation chunk (0 = kernel default: 48 with two planes, 24 with three)
-    f16: bool = False   # fp16 planes of weight * scale (the "h2" operand mode)
+    acc_chunk: int = 0  # MMAs per accumulation chunk (0 = kernel default: 16 with one plane, 48 with two, 24 with three)
+    f16: bool = False   # fp16 planes of weight * scale (the "h2" / "h1" operand modes)
     scale: float = 1.0
 
 
 def split_host(w: torch.Tensor, planes=2):
-    """fp32 -> bf16 planes (or, planes == "h2", fp16 planes of w * F16_W_SCALE) with torch ops (load-time weight preparation only)."""
-    if planes == H2:
+    """fp32 -> bf16 planes (or, planes == "h2" / "h1", two / one fp16 planes of w * F16_W_SCALE) with torch ops (load-time
+    weight preparation only)."""
+    if planes in (H2, H1):
         assert float(w.abs().max()) * F16_W_SCALE < 6.0e4, "weight too large for the fp16 plane scale"
         ws = w * F16_W_SCALE
         hi = ws.to(torch.float16)
-        return hi, (ws - hi.float()).to(torch.float16)
+        return (hi,) if planes == H1 else (hi, (ws - hi.float()).to(torch.float16))
     hi = w.to(torch.bfloat16)
     r = w - hi.float()
     lo = r.to(torch.bfloat16)
@@ -137,6 +146,8 @@ def pack_conv_weight(w: torch.Tensor, device=None, in_perm: Optional[torch.Tenso
     wp[:, :co] = w.permute(2, 3, 4, 0, 1).reshape(kd * kh * kw, co, ci).cpu()
     pl = split_host(wp, planes)
     dev = device or "cuda"
+    if planes == H1:
+        return PackedConvWeight(pl[0].contiguous().to(dev), None, co, co_pad, ci, (kd, kh, kw), None, 0, True, F16_W_SCALE)
     if planes == H2:
         return PackedConvWeight(pl[0].contiguous().to(dev), pl[1].contiguous().to(dev), co, co_pad, ci, (kd, kh, kw), None, ACC_CHUNK_F16,
                                 True, F16_W_SCALE)
@@ -178,15 +189,18 @@ def fold_poolconv_weight(w: torch.Tensor) -> torch.Tensor:
     return 0.25 * w4
 
 
-def pack_upconv_weight(w: torch.Tensor, device=None, planes: int = 2) -> PackedConvWeight:
+def pack_upconv_weight(w: torch.Tensor, device=None, planes=2) -> PackedConvWeight:
     """OIHW 3x3 fp32 (already SN/WS-folded) -> phase-folded PackedConvWeight [16 = phase*4 + ty*2 + tx][Cout][Cin] for
-    conv_igemm(..., upconv=True).  Cout must be a multiple of 32 (no padding rows; pair-mode N tiles)."""
-    assert planes == 2, "the sub-pixel convolution runs with two-plane operands"
+    conv_igemm(..., upconv=True).  Cout must be a multiple of 32 (no padding rows; pair-mode N tiles).  planes: 2 (bf16) or H1."""
+    assert planes in (2, H1), "the sub-pixel convolution runs with two bf16 planes or one fp16 plane"
     co, ci = w.shape[:2]
     assert co % 32 == 0 and ci % 64 == 0, (co, ci)
     wp = fold_upconv_weight(w).reshape(16, co, ci).contiguous()
-    hi, lo = split_host(wp, 2)
     dev = device or "cuda"
+    if planes == H1:
+        (hi,) = split_host(wp, H1)
+        return PackedConvWeight(hi.contiguous().to(dev), None, co, co, ci, (1, 3, 3), None, 0, True, F16_W_SCALE)
+    hi, lo = split_host(wp, 2)
     return PackedConvWeight(hi.contiguous().to(dev), lo.contiguous().to(dev), co, co, ci, (1, 3, 3), None, ACC_CHUNK_BF16)
 
 
@@ -195,13 +209,15 @@ def pack_upconv_weight(w: torch.Tensor, device=None, planes: int = 2) -> PackedC
 # ------------------------------------------------------------------------------------------------
 def grid_sample3d(inp: torch.Tensor, grid: Optional[torch.Tensor] = None, theta: Optional[torch.Tensor] = None,
                   out_size=None, in_layout: str = "ncdhw", out_layout: Optional[str] = None, want_f32: bool = True,
-                  want_split: bool = False, planes: int = 2):
+                  want_split: bool = False, planes=2):
     """Trilinear, zeros padding, align_corners=False (va.py:261-265).
 
     in_layout  'ncdhw' (N,C,D,H,W)  or 'cl' (N,D,H,W,C)
     out_layout 'ncdhw' | 'cl' | 'hwdc' ((N,H,W,D,C): the decoder's flattened-2D layout); default = in_layout
     grid (N,Do,Ho,Wo,3) xyz, or theta (N,3,4) with out_size=(Do,Ho,Wo) for the fused affine lattice.
+    want_split: also the operand planes of the output (planes 2 / 3 bf16, or H1: one fp16 plane of y * F16_ACT_SCALE).
     """
+    assert planes in (2, 3, H1), "grid_sample3d writes two or three bf16 planes or one fp16 plane"
     _chk(inp)
     if in_layout == "ncdhw":
         N, Cc, Di, Hi, Wi = inp.shape
@@ -236,7 +252,8 @@ def grid_sample3d(inp: torch.Tensor, grid: Optional[torch.Tensor] = None, theta:
         return out if want_f32 else sp
     d = L.GridSample3dDesc(_p(inp), 1 if in_layout == "cl" else 0, N, Cc, Di, Hi, Wi, _p(grid), _p(theta), Do, Ho, Wo,
                            _p(out), _p(sp.hi) if sp else None, _p(sp.lo) if sp else None, os_["n"], os_["c"],
-                           os_["d"], os_["h"], os_["w"], _p(sp.lo2) if sp else None)
+                           os_["d"], os_["h"], os_["w"], _p(sp.lo2) if sp else None,
+                           1 if (sp is not None and sp.f16) else 0, sp.scale if (sp is not None and sp.f16) else 0.0)
     L.call("emo_grid_sample3d", C.byref(d), _stream())
     if want_f32 and want_split:
         return out, sp
@@ -377,7 +394,7 @@ def gn_head(x: torch.Tensor, gn: dict, w: torch.Tensor, bias: Optional[torch.Ten
 
 
 def split_bf16(x: torch.Tensor, planes=2) -> Split:
-    """fp32 -> operand planes (bf16 x2 / x3, or fp16 x2 of x * F16_ACT_SCALE when planes == "h2")"""
+    """fp32 -> operand planes (bf16 x2 / x3, or fp16 x2 / x1 of x * F16_ACT_SCALE when planes == "h2" / "h1")"""
     _chk(x)
     sp = Split.empty(x.shape, x.device, planes)
     if sp.f16:
@@ -415,7 +432,7 @@ class ConvProfiler:
     def summary(self):
         torch.cuda.synchronize()
         ms = sum(r[0].elapsed_time(r[1]) for r in self.rec)
-        self.mma_flops = sum(r[2] * r[3] for r in self.rec)  # bf16 MMA flops actually issued (3 or 6 per product)
+        self.mma_flops = sum(r[2] * r[3] for r in self.rec)  # MMA flops actually issued (1, 3 or 6 per product)
         return ms, sum(r[2] for r in self.rec), len(self.rec)
 
     def table(self):
@@ -447,7 +464,9 @@ def _conv_desc(a: Split, w: PackedConvWeight, stride, pad, bias, residual, res_s
     three = a.lo2 is not None
     assert not three or w.lo2 is not None, "3-plane activations need 3-plane weights (pack_conv_weight(planes=3))"
     assert a.f16 == w.f16, "fp16-plane activations need fp16-plane weights (pack_conv_weight(planes='h2')) and vice versa"
-    assert not (a.f16 and upconv), "the sub-pixel convolution runs with bf16 planes"
+    one = a.lo is None
+    assert one == (w.lo is None), "one-plane activations need one-plane weights (planes='h1') and vice versa"
+    assert not (a.f16 and upconv and not one), "the sub-pixel convolution runs with two bf16 planes or one fp16 plane"
     kd, kh, kw = w.k
     if pad is None:
         pad = (kd // 2, kh // 2, kw // 2)
@@ -476,8 +495,8 @@ def _conv_desc(a: Split, w: PackedConvWeight, stride, pad, bias, residual, res_s
         ret = (pout, psp) if (wf and wsp) else (pout if wf else psp)
     # algorithmic flops of the convolution being computed; MMA passes actually issued per algorithmic product
     # (sub-pixel mode issues 4 of the 9 taps)
-    prof = (2.0 * N * Do * Ho * Wo * w.cout * Ci * kd * kh * kw, (6 if three else 3) * (4.0 / 9.0 if upconv else 1.0),
-            f"{N}x{Di}x{Hi}x{Wi}x{Ci}->{w.cout} k{kd}{kh}{kw} s{stride[1]} p{'h2' if a.f16 else (3 if three else 2)}"
+    prof = (2.0 * N * Do * Ho * Wo * w.cout * Ci * kd * kh * kw, (6 if three else 1 if one else 3) * (4.0 / 9.0 if upconv else 1.0),
+            f"{N}x{Di}x{Hi}x{Wi}x{Ci}->{w.cout} k{kd}{kh}{kw} s{stride[1]} p{('h1' if one else 'h2') if a.f16 else (3 if three else 2)}"
             + (" up2-subpixel" if upconv else ""))
     return d, ret, pd, prof
 

@@ -35,7 +35,8 @@ extern "C" {
 enum { EMO_ACT_NONE = 0, EMO_ACT_RELU = 1, EMO_ACT_SIGMOID = 2, EMO_ACT_TANH = 3 };
 
 const char* emo_last_error(void);
-int emo_version(void); /* 105: + emo_conv_plan; 104: + emo_composite; 103: emo_conv_desc.post; 102: + emo_u8_to_image, emo_image_to_u8, emo_resize_bicubic; 101: emo_pose_desc and emo_conv_desc gained trailing fields */
+int emo_version(void); /* 106: one-plane fp16 operands (emo_conv_desc, emo_apply_desc, emo_grid_sample3d_desc.plane_fp16,
+                          emo_split_f16 with lo == NULL) and the EMO_CONV_KERNEL_H1_* kernels; 105: + emo_conv_plan; 104: + emo_composite; 103: emo_conv_desc.post; 102: + emo_u8_to_image, emo_image_to_u8, emo_resize_bicubic; 101: emo_pose_desc and emo_conv_desc gained trailing fields */
 /* sm count, and cc major*10+minor of the current device */
 int emo_device_info(int* sm_count, int* cc);
 
@@ -58,6 +59,10 @@ typedef struct {
   /* output element strides (in elements) for n, c, d, h, w. */
   long long os_n, os_c, os_d, os_h, os_w;
   void* out_lo2;          /* optional third bf16 plane (with out_hi/out_lo) */
+  /* one-plane fp16 operand mode (see emo_conv_desc.operand_fp16): when plane_fp16 != 0, out_hi receives fp16(y * plane_scale)
+   * (plane_scale a power of two) and out_lo / out_lo2 must be NULL. */
+  int plane_fp16;
+  float plane_scale;
 } emo_grid_sample3d_desc;
 int emo_grid_sample3d(const emo_grid_sample3d_desc* d, void* stream);
 
@@ -146,7 +151,8 @@ typedef struct emo_apply_desc_s {
   const float* ada_w; /* [N][C] or NULL */
   const float* ada_b;
   /* fp16 two-plane operand mode (see emo_conv_desc.operand_fp16): when plane_fp16 != 0, out_hi/out_lo receive the fp16
-   * planes of y * plane_scale (plane_scale a power of two that keeps the planes in fp16's normal range; out_lo2 unused). */
+   * planes of y * plane_scale (plane_scale a power of two that keeps the planes in fp16's normal range; out_lo2 unused).
+   * With out_lo == NULL only out_hi is written: the one-plane fp16 operand fp16(y * plane_scale). */
   int plane_fp16;
   float plane_scale;
 } emo_apply_desc;
@@ -224,7 +230,10 @@ typedef struct {
    * powers of two chosen by the caller (emo_apply.plane_scale / the weight packer); the kernel issues the same three MMAs
    * (hi*hi + hi*lo + lo*hi, kind::f16 with fp16 inputs) and multiplies the fp32 sums by out_scale = 1 / (sa * sw) before
    * bias / residual.  ~22 mantissa bits per operand: fp32-faithful like the three-plane bf16 mode at half its MMAs.
-   * Not combinable with a_lo2/w_lo2 or upconv. */
+   * Not combinable with a_lo2/w_lo2 or upconv.
+   * One-plane fp16 operands: operand_fp16 with a_lo == w_lo == NULL (and no a_lo2/w_lo2).  a_hi / w_hi are fp16(activation * sa)
+   * and fp16(weight * sw); ONE MMA per product (~2^-11 relative per operand: decoder-only, DESIGN.md section 2).  Also
+   * combinable with upconv (w_hi then holds the phase-folded weights). */
   int operand_fp16;
   float out_scale;
   /* optional post-op on the convolution's output: y = act(GN-or-affine(out) [+ res*A2 + B2]) -> fp32 and/or operand planes,
@@ -246,7 +255,11 @@ enum {
   EMO_CONV_KERNEL_BF16X3_KC32 = 3, /* conv_igemm_kernel<32, 3> */
   EMO_CONV_KERNEL_F16_KC64 = 4,    /* conv_igemm_f16_kernel<64, 2> */
   EMO_CONV_KERNEL_F16_KC32 = 5,    /* conv_igemm_f16_kernel<32, 2> */
-  EMO_CONV_KERNEL_UPCONV_KC64 = 6  /* conv_igemm_ps_kernel<64, 2> */
+  EMO_CONV_KERNEL_UPCONV_KC64 = 6, /* conv_igemm_ps_kernel<64, 2> */
+  /* one-plane fp16 operands (operand_fp16 with a_lo == w_lo == NULL), reported with NP = 1; ids 7, 8, 9 */
+  EMO_CONV_KERNEL_H1_KC64,         /* conv_igemm_f16_kernel<64, 1> */
+  EMO_CONV_KERNEL_H1_KC32,         /* conv_igemm_f16_kernel<32, 1> */
+  EMO_CONV_KERNEL_H1_UPCONV_KC64   /* conv_igemm_ps_f16_kernel<64, 1> */
 };
 enum {
   EMO_CONV_FINISH_NONE = 0,           /* the convolution kernel writes the output */
@@ -361,7 +374,8 @@ int emo_pose_theta(const emo_pose_desc* d, void* stream);
 
 /* fp32 -> bf16 hi/lo(/lo2) planes (n elements); lo2 may be NULL. */
 int emo_split_bf16(const float* x, long long n, void* hi, void* lo, void* lo2, void* stream);
-/* fp32 -> fp16 hi/lo planes of x * scale (n elements), the operand format of emo_conv_desc.operand_fp16. */
+/* fp32 -> fp16 hi/lo planes of x * scale (n elements), the operand format of emo_conv_desc.operand_fp16.  lo == NULL: the
+ * one-plane operand fp16(x * scale) only. */
 int emo_split_f16(const float* x, long long n, float scale, void* hi, void* lo, void* stream);
 /* ------------------------------------------------------------------------------------------------
  * Pre/post-processing at the wrapper boundary (SURVEY.md §8f-2).

@@ -1,0 +1,215 @@
+#!/usr/bin/env python
+"""Exact vs fast mode (decoder on one fp16 operand plane, ops.H1) in the same run on the same card; one JSON line.
+
+    python tools/fast_mode_bench.py [--steps K] [--warmup W] [--rounds R]
+
+Per mode, with bench.py's definitions (driver frame @512^2, shipped model, synthetic seed-0 weights, cached source identity):
+  fps          device-resident driver frames/s, four captured frames in flight (infer.DriverPipeline depth 4), CUDA events
+  e2e          frames/s with a pinned host frame in and the host image out every step (two frames of host run-ahead per stream)
+  latency_ms   one captured frame at a time (depth 1), CUDA events / K
+  decoder_conv_ms_graph  the decoder's convolutions per frame: every conv shape of one decoder pass as CUDA-graph replays of 10
+               back-to-back launches (mean of the no-residual / residual forms, as bench.py times the frame's convs), weighted
+               by its launches per frame
+  decoder_ms_graph       one whole decoder pass, CUDA-graph replays
+The modes alternate for `--rounds` rounds so that a drift of the card's clocks hits both; the median of the rounds is
+reported, with the spread.  The SM clocks during the timed regions are recorded as bench.py records them."""
+from __future__ import annotations
+
+import argparse
+import json
+import math
+import pathlib
+import re
+import statistics
+import subprocess
+import sys
+import time
+
+import torch
+
+ROOT = pathlib.Path(__file__).resolve().parents[1]
+sys.path.insert(0, str(ROOT))
+
+import bench  # noqa: E402  (frame(), ClockSampler, SIZE: the benchmark's own definitions)
+
+
+def graph_time_conv(shape_key: str, reps: int = 10):
+    """bench.graph_time_conv for every operand mode of the profiler's shape keys (p2 / p3 / ph2 / ph1)"""
+    from emoportraits_b200 import ops
+
+    m = re.match(r"(\d+)x(\d+)x(\d+)x(\d+)x(\d+)->(\d+) k(\d)(\d)(\d) s(\d) p(\w+)( up2-subpixel)?", shape_key)
+    N, D, H, W, Ci, Co, kd, kh, kw, st_ = map(int, m.groups()[:10])
+    pl, up = m.group(11), m.group(12)
+    planes = {"h2": ops.H2, "h1": ops.H1}.get(pl) or int(pl)
+    x = torch.randn((N, D, H, W, Ci), device="cuda")
+    w = torch.randn((Co, Ci, kd, kh, kw) if kd > 1 else (Co, Ci, kh, kw)) / math.sqrt(Ci * kd * kh * kw)
+    a = ops.split_bf16(x, planes)
+    pw = ops.pack_upconv_weight(w, planes=planes) if up else ops.pack_conv_weight(w, planes=planes)
+    pad = (kd // 2, 1, 1) if kh == 4 else None
+    Ho, Wo = (2 * H, 2 * W) if up else ((H + 2 * (1 if kh == 4 else kh // 2) - kh) // st_ + 1, (W + 2 * (1 if kw == 4 else kw // 2) - kw) // st_ + 1)
+    out = torch.empty((N, D, Ho, Wo, Co), device="cuda")
+    bias = torch.zeros(Co, device="cuda")
+    res_full = torch.randn(out.shape, device="cuda") if Co % 4 == 0 else None
+    times = []
+    for res in (None, res_full):
+        ops.begin_pass("cuda")
+        stt = ops.new_stats(N, 32, "cuda") if Co % 32 == 0 else None
+        run = lambda: ops.conv_igemm(a, pw, stride=(1, st_, st_), pad=pad, out=out, bias=bias, residual=res, stats=stt, upconv=bool(up))
+        times.append(_graph_us(run, reps))
+    return sum(times) / len(times)
+
+
+def _graph_us(run, reps, replays=5):
+    for _ in range(2):
+        run()
+    torch.cuda.synchronize()
+    g = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(g):
+        for _ in range(reps):
+            run()
+    g.replay()
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(replays):
+        g.replay()
+    e1.record()
+    torch.cuda.synchronize()
+    return e0.elapsed_time(e1) / (replays * reps) * 1000.0
+
+
+def decoder_times(model):
+    """(graph-timed decoder conv ms per frame, graph-timed whole decoder ms, per-shape table)"""
+    from emoportraits_b200 import ops
+
+    cfg, dec = model.cfg, model.decoder_nw
+    feat = ops.split_bf16(torch.rand((1, 1, cfg.S, cfg.S, cfg.D * cfg.C), device="cuda"), dec.planes)
+    prof = ops.ConvProfiler()
+    ops.set_conv_profiler(prof)
+    ops.begin_pass("cuda")
+    dec(feat)
+    torch.cuda.synchronize()
+    ops.set_conv_profiler(None)
+    table, conv_us = [], 0.0
+    for name, n, _ms, _alg, _mma in prof.table():
+        us = graph_time_conv(name)
+        conv_us += us * n
+        table.append({"shape": name, "launches": n, "us_per_launch": us})
+
+    def whole():
+        ops.begin_pass("cuda")
+        dec(feat)
+    dec_us = _graph_us(whole, 1, replays=20)
+    return conv_us / 1000.0, dec_us / 1000.0, table
+
+
+def measure(model, st, frames_host, frames_dev, K, W):
+    from emoportraits_b200.infer import DriverPipeline
+
+    out = {}
+    pipe = DriverPipeline(model, st, depth=4, mix=True)
+    for i in range(W):
+        pipe.submit(frames_dev[i % len(frames_dev)])
+    pipe.drain()
+    torch.cuda.synchronize()
+    sampler = bench.ClockSampler(torch.cuda.current_device())
+    sampler.start()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for i in range(K):
+        pipe.submit(frames_dev[i % len(frames_dev)])
+    pipe.drain()
+    e1.record()
+    torch.cuda.synchronize()
+    out["fps"] = K / (e0.elapsed_time(e1) / 1000.0)
+    out["clocks"] = sampler.stop()
+    ring = 8
+    hosts = [torch.empty((1, 3, bench.SIZE, bench.SIZE)).pin_memory() for _ in range(ring)]
+    tickets = [None] * ring
+
+    def step_e2e(i):
+        t = tickets[i % ring]
+        if t is not None:
+            t.done.synchronize()
+        tickets[i % ring] = pipe.submit(frames_host[i % len(frames_host)], host_out=hosts[i % ring])
+
+    for i in range(2 * ring):
+        step_e2e(i)
+    pipe.drain()
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    for i in range(K):
+        step_e2e(i)
+    pipe.drain()
+    torch.cuda.synchronize()
+    out["e2e"] = K / (time.perf_counter() - t0)
+    del pipe
+    lat = DriverPipeline(model, st, depth=1, mix=True)
+    for i in range(3):
+        lat.submit(frames_dev[i % len(frames_dev)])
+    lat.drain()
+    torch.cuda.synchronize()
+    e0.record()
+    for i in range(K):
+        lat.submit(frames_dev[i % len(frames_dev)])
+    lat.drain()
+    e1.record()
+    torch.cuda.synchronize()
+    out["latency_ms"] = e0.elapsed_time(e1) / K
+    return out
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=200)
+    ap.add_argument("--warmup", type=int, default=10)
+    ap.add_argument("--rounds", type=int, default=3)
+    args = ap.parse_args()
+    assert torch.cuda.is_available(), "tools/fast_mode_bench.py measures on the GPU"
+    from emoportraits_b200.checkpoint import synthetic_head_pose_state_dict, synthetic_state_dict
+    from emoportraits_b200.config import shipped_config
+    from emoportraits_b200.infer import Model
+
+    cfg = shipped_config(bench.SIZE)
+    sd, hsd = synthetic_state_dict(cfg, 0), synthetic_head_pose_state_dict(0)
+    models = {m: Model(cfg, sd, hsd, "cuda", precision=m) for m in ("exact", "fast")}
+    src = bench.frame(bench.SIZE, 0).cuda()
+    states = {m: models[m].source_pass(src) for m in models}
+    frames_host = [bench.frame(bench.SIZE, 1000 + i).pin_memory() for i in range(8)]
+    frames_dev = [f.cuda() for f in frames_host]
+    K, W = args.steps, max(args.warmup, 3)
+    runs = {m: [] for m in models}
+    for _ in range(args.rounds):
+        for m in models:
+            runs[m].append(measure(models[m], states[m], frames_host, frames_dev, K, W))
+    res = {}
+    for m, rs in runs.items():
+        conv_ms, dec_ms, table = decoder_times(models[m])
+        res[m] = {k: statistics.median(r[k] for r in rs) for k in ("fps", "e2e", "latency_ms")}
+        res[m].update({f"{k}_runs": [r[k] for r in rs] for k in ("fps", "e2e", "latency_ms")})
+        res[m].update(decoder_conv_ms_graph=conv_ms, decoder_ms_graph=dec_ms, decoder_conv_shapes=table,
+                      clocks=[r["clocks"] for r in rs])
+    # the same driver frame through both modes: how far fast mode moves the image
+    with torch.no_grad():
+        img = {m: models[m].driver_pass(states[m], frames_dev[0], mix=True)[0] for m in models}
+    d = (img["fast"] - img["exact"]).abs()
+    props = torch.cuda.get_device_properties(0)
+    line = {
+        "metric": "fast mode (decoder on one fp16 operand plane) vs exact, driver frames @512^2",
+        "gpu": props.name, "sm_count": props.multi_processor_count, "steps": K, "warmup": W, "rounds": args.rounds,
+        "exact": res["exact"], "fast": res["fast"],
+        "speedup": {k: (res["fast"][k] / res["exact"][k]) if k != "latency_ms" else res["exact"][k] / res["fast"][k]
+                    for k in ("fps", "e2e", "latency_ms")},
+        "decoder_conv_speedup_graph": res["exact"]["decoder_conv_ms_graph"] / res["fast"]["decoder_conv_ms_graph"],
+        "image_vs_exact": {"max_abs": d.max().item(), "mean_abs": d.mean().item()},
+    }
+    try:
+        line["power_limit"] = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader"],
+                                             capture_output=True, text=True, timeout=30).stdout.strip()
+    except (OSError, subprocess.SubprocessError):
+        line["power_limit"] = None
+    print(json.dumps(line))
+
+
+if __name__ == "__main__":
+    main()
