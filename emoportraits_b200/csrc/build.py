@@ -16,7 +16,7 @@ import sys
 HERE = pathlib.Path(__file__).resolve().parent
 LIB = HERE / "libemoport.so"
 SOURCES = ["conv_igemm.cu", "grid_sample.cu", "norm.cu", "misc.cu", "masks.cu"]
-HEADERS = ["common.cuh", "pose_math.cuh", "wgmma.cuh", "conv_igemm_kernel.inc", "apply_kernel.inc", "../../include/emoportraits_b200.h"]
+HEADERS = ["common.cuh", "pose_math.cuh", "wgmma.cuh", "../../include/emoportraits_b200.h"]
 ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]
 
 

@@ -65,13 +65,13 @@ struct ConvKParams {
   int out_nchw;
   double* stats;
   int G, cpg;
-  // sub-pixel mode (conv_igemm_ps_kernel): 3x3 conv over the nearest-x2 upsampling of the input, evaluated on the LOW-resolution
+  // sub-pixel mode (the PS kernels): 3x3 conv over the nearest-x2 upsampling of the input, evaluated on the LOW-resolution
   // planes.  Dout/Hout/Wout above then describe the low-resolution pixel grid the tiles walk; the output tensor is
   // [N][Dout][oH = 2 Hout][oW = 2 Wout][Cout].  The N-tile index carries the output phase: nt = phase * ntc + channel tile,
   // phase = 2 * (row parity) + (column parity); each phase has its own four 2x2 taps (weights [phase * 4 + tap]).
   int oH, oW;
   int ntc;  // channel tiles per phase (= Cout_pad / BN)
-  float out_scale;  // conv_igemm_f16_kernel: 1 / (activation plane scale * weight plane scale)
+  float out_scale;  // fp16 operands (the F16 kernels): 1 / (activation plane scale * weight plane scale)
   // row-reuse mode (stride-1 convolutions with kh > 1 on tiles of one depth slice): the A operand of a (kernel column,
   // k-chunk) group is ONE halo tile of a_rows = tw * (th + kh - 1) pixels serving all kh tap rows; A ring of `sa` halo tiles,
   // B ring of `sb` weight tiles (see the kernel's producer role)
@@ -195,30 +195,503 @@ struct TMaps {
   CUtensorMap b[3];  // weight planes
 };
 
-#define EMO_CONV_PS 0
-#define EMO_CONV_F16 0
-#define EMO_CONV_KERNEL_NAME conv_igemm_kernel
-#include "conv_igemm_kernel.inc"
-#undef EMO_CONV_PS
-#undef EMO_CONV_KERNEL_NAME
-#define EMO_CONV_PS 1
-#define EMO_CONV_KERNEL_NAME conv_igemm_ps_kernel
-#include "conv_igemm_kernel.inc"
-#undef EMO_CONV_PS
-#undef EMO_CONV_F16
-#undef EMO_CONV_KERNEL_NAME
-#define EMO_CONV_PS 0
-#define EMO_CONV_F16 1
-#define EMO_CONV_KERNEL_NAME conv_igemm_f16_kernel
-#include "conv_igemm_kernel.inc"
-#undef EMO_CONV_PS
-#undef EMO_CONV_KERNEL_NAME
-#define EMO_CONV_PS 1
-#define EMO_CONV_KERNEL_NAME conv_igemm_ps_f16_kernel
-#include "conv_igemm_kernel.inc"
-#undef EMO_CONV_PS
-#undef EMO_CONV_F16
-#undef EMO_CONV_KERNEL_NAME
+// The convolution kernel proper.  The host's instantiation table (kConvKernels) lists the forms that exist:
+//   PS = false, F16 = false   the kernel of every ordinary convolution
+//   F16 = true                fp16 operand planes (emo_conv_desc.operand_fp16): fp16 wgmma instead of bf16 and a power-of-two
+//       rescale of the finished sums
+//   PS = true                 sub-pixel form of `nearest x2 -> 3x3 conv` (emo_conv_desc.upconv):
+//       the tiles walk the LOW-resolution pixel grid (p.Hout x p.Wout); the N-tile index carries the output phase
+//       (nt = phase * p.ntc + channel tile, phase = 2 * row parity + column parity); each phase has four 2x2 taps on the
+//       low-resolution planes (weights [phase * 4 + tap]) and its results land on the pixels of that parity of the
+//       [p.oH = 2 p.Hout][p.oW = 2 p.Wout] output.
+//   PS = true, F16 = true     the sub-pixel form on one fp16 plane
+// KC = channels per k-chunk (64 or 32).
+// NP = number of 16-bit planes per operand: 1 -> 1 product (fp16 only, ~2^-11 relative per operand), 2 -> 3 products
+// (~2^-16 relative with bf16, ~2^-22 with fp16), 3 -> 6 products (~2^-24, fp32-faithful)
+// Three warpgroups: warps 0..7 are two consumer warpgroups (warpgroup w issues the wgmmas of tile rows 64 w .. 64 w + 63, promotes its
+// accumulation chunks to fp32 registers and runs the final phase of those rows), warp 8 is the TMA producer; setmaxnreg moves
+// the registers of the producer warpgroup to the consumers (acc + chunk = 2 x BN/2 fp32 per thread).
+// Final phase in registers: bias (as the accumulation's starting value), residual, activation, post-add, float2 stores of the
+// wgmma fragment (two rows x two adjacent channels per 8-channel block), GroupNorm statistics by shuffle reduction.
+template <int KC, int NP, bool PS, bool F16>
+__global__ void __launch_bounds__(kThreads, 1)
+conv_igemm_kernel(const __grid_constant__ TMaps tm, const __grid_constant__ ConvKParams p) {
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  // dynamic smem is only guaranteed 16B-aligned by the API; realign to 1024 for the swizzle atoms.
+  uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
+
+  const int BN = p.BN;
+  const uint32_t a_bytes = kTileM * KC * 2;
+  const uint32_t b_bytes = (uint32_t)BN * KC * 2;
+  const uint32_t stage_bytes = NP * a_bytes + NP * b_bytes;
+  const int S = p.stages;
+
+  // Row-reuse mode (p.yreuse, see the producer): instead of S stages of {A tile, B tile} per (tap, k-chunk) the operand area
+  // holds an A ring of p.sa halo tiles (th + kh - 1 image rows: ONE load serves the kh taps of a kernel column) followed by a
+  // B ring of p.sb weight tiles.
+  const uint32_t a_halo_plane = (uint32_t)p.a_rows * KC * 2;  // one plane of a halo tile
+  const uint32_t a_halo_bytes = NP * a_halo_plane;
+  const uint32_t b_tile_bytes = NP * b_bytes;
+  uint8_t* b_ring = smem + (size_t)p.sa * a_halo_bytes;
+  uint8_t* tail = smem + (p.yreuse ? (size_t)p.sa * a_halo_bytes + (size_t)p.sb * b_tile_bytes : (size_t)S * stage_bytes);
+  uint64_t* full_bar = (uint64_t*)tail;
+  uint64_t* empty_bar = full_bar + kMaxStages;
+  uint64_t* afull_bar = empty_bar + kMaxStages;  // row-reuse mode: A ring (full_bar / empty_bar then serve the B ring)
+  uint64_t* aempty_bar = afull_bar + kMaxAStages;
+  // tile statistics: one slot per (consumer warp, column); every slot has exactly ONE writer per tile, so the CTA's column sums
+  // are plain stores summed in a fixed order afterwards (no atomics inside the CTA: reproducible run to run)
+  float* col_sum = (float*)(aempty_bar + kMaxAStages);  // [kConsumerWarps][kMaxBN]
+  float* col_sq = col_sum + kConsumerWarps * kMaxBN;     // [kConsumerWarps][kMaxBN]
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  EMO_STAMP(0, threadIdx.x == 0);
+
+  if (warp == kConsumerWarps) {
+    // barrier initialisation and descriptor prefetches spread over the lanes of the producer warp
+    if (lane < NP) {
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&tm.a[lane]) : "memory");
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&tm.b[lane]) : "memory");
+    }
+    const int nring = p.yreuse ? p.sb : S;
+    if (lane < nring) {
+      mbar_init(&full_bar[lane], 1);
+      mbar_init(&empty_bar[lane], (uint32_t)kConsumerWarps);  // one arrival per consumer warp
+    }
+    if (lane >= 16 && lane < 16 + kMaxAStages) {
+      mbar_init(&afull_bar[lane - 16], 1);
+      mbar_init(&aempty_bar[lane - 16], (uint32_t)kConsumerWarps);
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");  // every initialising lane publishes its own barriers
+  }
+  for (int i = threadIdx.x; i < 2 * kConsumerWarps * kMaxBN; i += kThreads) col_sum[i] = 0.f;
+  __syncthreads();
+  EMO_STAMP(1, threadIdx.x == 0);
+  const int tile_first = (int)blockIdx.x;
+  const int tile_step = (int)gridDim.x;
+  const int ksplit = p.ksplit;  // work item = tile * ksplit + part (ksplit == 1: item == tile)
+
+  const int taps = p.kd * p.kh * p.kw;
+  const int ksteps = taps * p.kchunks;
+  const int total_tiles = p.m_tiles * p.n_tiles * p.ksplit;  // work items
+  const int rows_a = p.tw * p.th * p.td;
+  const uint32_t tx_bytes = (uint32_t)NP * ((uint32_t)rows_a * KC * 2 + b_bytes);
+
+  if (warp >= kConsumerWarps) {
+    // the producer warpgroup hands its registers to the consumers; its warps 1..3 have nothing to do
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kProducerRegs));
+    if (warp != kConsumerWarps) return;
+    // ===================== TMA producer (whole warp walks the loop; one elected lane issues) =====================
+    if (p.yreuse) {
+      // Row reuse: for a stride-1 convolution the kh taps of one kernel column read the SAME pixels shifted by whole image
+      // rows, and in the [row][column][channel] tile a row shift is a whole-swizzle-atom offset (tw x KC x 2 bytes, a multiple
+      // of 1024).  So the A operand of a (kernel column, k-chunk) group is loaded ONCE as a halo tile of th + kh - 1 rows and
+      // the wgmmas of tap row b read it through a descriptor advanced by b x tw rows: kh times less activation traffic from L2
+      // and fewer shared-memory writes per k-step.
+      EMO_STAMP(2, lane == 0);
+      int sa = 0, sb = 0;
+      uint32_t pha = 0, phb = 0;
+      const uint32_t a_tx = (uint32_t)NP * a_halo_plane, b_tx = (uint32_t)NP * b_bytes;
+      const int ngroups = p.kd * p.kw * p.kchunks;
+      for (int item = tile_first; item < total_tiles; item += tile_step) {
+        const int nt = item / p.m_tiles;
+        int mt = item - nt * p.m_tiles;
+        const int twi = mt % p.tiles_w; mt /= p.tiles_w;
+        const int thi = mt % p.tiles_h; mt /= p.tiles_h;
+        const int tdi = mt % p.tiles_d; mt /= p.tiles_d;
+        const int n = mt;
+        const int x0 = twi * p.tw - p.pw, y0 = thi * p.th - p.ph, z0 = tdi * p.td - p.pd;
+        const int ph = PS ? nt / p.ntc : 0;  // output phase of the sub-pixel form
+        const int n0 = (nt - ph * p.ntc) * BN;
+        const int xs = (ph & 1) ? 1 : 0, ys = (ph >> 1) ? 1 : 0;
+        for (int gi = 0; gi < ngroups; ++gi) {
+          const int kc = gi % p.kchunks;
+          const int t = gi / p.kchunks;
+          const int c = t % p.kw, a = t / p.kw;
+          mbar_wait(&aempty_bar[sa], pha ^ 1);
+          if (!elect_one()) {
+          }
+#ifdef EMO_CONV_DEBUG
+          else if (p.dbg & 1) {
+            mbar_expect_tx(&afull_bar[sa], 0);
+          }
+#endif
+          else {
+            uint8_t* dst = smem + (size_t)sa * a_halo_bytes;
+            mbar_expect_tx(&afull_bar[sa], a_tx);
+#pragma unroll
+            for (int pl = 0; pl < NP; ++pl) tma_load_5d(&tm.a[pl], &afull_bar[sa], dst + pl * a_halo_plane, kc * KC, x0 + xs + c, y0 + ys, z0 + a, n);
+          }
+          __syncwarp();
+          if (++sa == p.sa) { sa = 0; pha ^= 1; }
+          for (int b = 0; b < p.kh; ++b) {
+            const int wtap = PS ? ph * 4 + b * 2 + c : (a * p.kh + b) * p.kw + c;
+            mbar_wait(&empty_bar[sb], phb ^ 1);
+            if (!elect_one()) {
+            }
+#ifdef EMO_CONV_DEBUG
+            else if (p.dbg & 1) {
+              mbar_expect_tx(&full_bar[sb], 0);
+            }
+#endif
+            else {
+              uint8_t* dst = b_ring + (size_t)sb * b_tile_bytes;
+              mbar_expect_tx(&full_bar[sb], b_tx);
+#pragma unroll
+              for (int pl = 0; pl < NP; ++pl) tma_load_3d(&tm.b[pl], &full_bar[sb], dst + pl * b_bytes, kc * KC, n0, wtap);
+            }
+            __syncwarp();
+            if (++sb == p.sb) { sb = 0; phb ^= 1; }
+          }
+        }
+      }
+      EMO_STAMP(3, lane == 0);
+    } else {
+      EMO_STAMP(2, lane == 0);
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int item = tile_first; item < total_tiles; item += tile_step) {
+        const int tile = item / ksplit, part = item - tile * ksplit;
+        const int ks0 = (int)((long long)ksteps * part / ksplit), ks1 = (int)((long long)ksteps * (part + 1) / ksplit);
+        const int nt = tile / p.m_tiles;
+        int mt = tile - nt * p.m_tiles;
+        const int twi = mt % p.tiles_w; mt /= p.tiles_w;
+        const int thi = mt % p.tiles_h; mt /= p.tiles_h;
+        const int tdi = mt % p.tiles_d; mt /= p.tiles_d;
+        const int n = mt;
+        const int x0 = twi * p.tw * p.sw - p.pw;
+        const int y0 = thi * p.th * p.sh - p.ph;
+        const int z0 = tdi * p.td * p.sd - p.pd;
+        // sub-pixel form: phase (row parity, column parity) of the output lattice: taps at low-res offsets {-1, 0} for parity 0
+        // and {0, +1} for parity 1 (kh = kw = 2 in this mode), weights of this phase at [phase * 4 + tap]
+        const int ph = PS ? nt / p.ntc : 0;
+        const int n0 = (nt - ph * p.ntc) * BN;
+        const int xs = (ph & 1) ? 1 : 0, ys = (ph >> 1) ? 1 : 0;  // p.pw = p.ph = 1: x0 + xs = tile origin - 1 or - 0
+        for (int ks = ks0; ks < ks1; ++ks) {
+          const int tap = ks / p.kchunks, kc = ks - tap * p.kchunks;
+          const int c = tap % p.kw + xs, b = (tap / p.kw) % p.kh + ys, a = PS ? 0 : tap / (p.kw * p.kh);
+          const int wtap = ph * 4 + tap;
+          mbar_wait(&empty_bar[stage], phase ^ 1);
+          uint8_t* st = smem + (size_t)stage * stage_bytes;
+          if (!elect_one()) {
+          }
+#ifdef EMO_CONV_DEBUG
+          else if (p.dbg & 1) {
+            mbar_expect_tx(&full_bar[stage], 0);
+          }
+#endif
+          else {
+            mbar_expect_tx(&full_bar[stage], tx_bytes);
+#pragma unroll
+            for (int pl = 0; pl < NP; ++pl) {
+              tma_load_5d(&tm.a[pl], &full_bar[stage], st + pl * a_bytes, kc * KC, x0 + c, y0 + b, z0 + a, n);
+              tma_load_3d(&tm.b[pl], &full_bar[stage], st + NP * a_bytes + pl * b_bytes, kc * KC, n0, wtap);
+            }
+          }
+          __syncwarp();
+          if (++stage == S) { stage = 0; phase ^= 1; }
+        }
+      }
+      EMO_STAMP(3, lane == 0);
+    }
+    return;
+  }
+
+  // ===================== consumer warpgroups =====================
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kConsumerRegs));
+  const int wg = warp >> 2;  // tile rows 64 wg .. 64 wg + 63
+  const int wq = warp & 3;   // 16-row slice of the warpgroup's rows
+  const int et = threadIdx.x;  // 0..255 among the consumer threads
+  const int cq = 2 * (lane & 3);  // first of this thread's two columns in every 8-column block
+  const int F = p.flush;
+  const uint32_t wg_off = (uint32_t)wg * 64u * KC * 2u;  // the warpgroup's 64 rows inside an A tile
+  // The wgmmas of one k-step (KC channels of one tap).  The tensor core accumulates with truncation, so an accumulator only
+  // ever takes a short chunk of MMAs (p.flush k-steps, started with scale-d = 0); every chunk is added to the fp32 sums in
+  // registers with round-to-nearest adds (DESIGN.md section 2).
+  float acc[kMaxBN / 2], cf[kMaxBN / 2];
+#pragma unroll
+  for (int j = 0; j < kMaxBN / 2; ++j) cf[j] = 0.f;
+  auto issue_kstep = [&](auto n_tile, uint32_t sa_, uint32_t a_plane, uint32_t sb_, bool first) {
+#ifdef EMO_CONV_DEBUG
+    if (p.dbg & 2) return;
+#endif
+    uint64_t dA[NP], dB[NP];
+#pragma unroll
+    for (int pl = 0; pl < NP; ++pl) {
+      dA[pl] = make_kmajor_desc<KC>(sa_ + pl * a_plane);
+      dB[pl] = make_kmajor_desc<KC>(sb_ + pl * b_bytes);
+    }
+    {
+      constexpr int N = decltype(n_tile)::value;
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < KC / 16; ++kk) {
+        const uint64_t adv = (uint64_t)(kk * 2);  // 16 elements = 32 B = 2 x 16B units
+        const uint32_t acc0 = (first && kk == 0) ? 0u : 1u;
+        if constexpr (NP == 1) {
+          wgmma<F16, N>(cf, dA[0] + adv, dB[0] + adv, acc0);
+        } else if constexpr (NP == 2) {
+          wgmma<F16, N>(cf, dA[1] + adv, dB[0] + adv, acc0);
+          wgmma<F16, N>(cf, dA[0] + adv, dB[1] + adv, 1u);
+          wgmma<F16, N>(cf, dA[0] + adv, dB[0] + adv, 1u);
+        } else {
+          // smallest terms first: lo2*hi, hi*lo2, lo*lo, lo*hi, hi*lo, hi*hi
+          wgmma<F16, N>(cf, dA[NP - 1] + adv, dB[0] + adv, acc0);
+          wgmma<F16, N>(cf, dA[0] + adv, dB[NP - 1] + adv, 1u);
+          wgmma<F16, N>(cf, dA[1] + adv, dB[1] + adv, 1u);
+          wgmma<F16, N>(cf, dA[1] + adv, dB[0] + adv, 1u);
+          wgmma<F16, N>(cf, dA[0] + adv, dB[1] + adv, 1u);
+          wgmma<F16, N>(cf, dA[0] + adv, dB[0] + adv, 1u);
+        }
+      }
+      wgmma_commit();
+    }
+  };
+  // One k-step stays in flight while the next is issued: a stage is released once the wgmmas that read it have completed
+  // (wait_group 1 after the next k-step's issue); the last k-step of a chunk drains the group before the promotion.
+  auto release = [&](uint64_t* bar) {
+    __syncwarp();
+    if (bar && lane == 0) mbar_arrive(bar);
+  };
+  auto finish_kstep = [&](bool chunk_last, uint64_t*& pend_b, uint64_t*& pend_a, uint64_t* cur_b, uint64_t* cur_a) {
+    if (chunk_last) {
+      wgmma_wait<0>();
+      wgmma_fence_operands<kMaxBN / 2>(cf);
+      release(pend_b); release(pend_a); release(cur_b); release(cur_a);
+      pend_b = pend_a = nullptr;
+#pragma unroll
+      for (int j = 0; j < kMaxBN / 2; ++j) acc[j] += cf[j];
+    } else {
+      wgmma_wait<1>();
+      release(pend_b); release(pend_a);
+      pend_b = cur_b; pend_a = cur_a;
+    }
+  };
+
+  int stage = 0, sa = 0, sb = 0;
+  uint32_t phase = 0, pha = 0, phb = 0;
+  for (int item = tile_first; item < total_tiles; item += tile_step) {
+    const int tile = item / ksplit, part = item - tile * ksplit;
+    const int nks = (int)((long long)ksteps * (part + 1) / ksplit) - (int)((long long)ksteps * part / ksplit);
+    const int nt = tile / p.m_tiles;
+    int mt = tile - nt * p.m_tiles;
+    const int twi = mt % p.tiles_w; mt /= p.tiles_w;
+    const int thi = mt % p.tiles_h; mt /= p.tiles_h;
+    const int tdi = mt % p.tiles_d; mt /= p.tiles_d;
+    const int n = mt;
+    const int ph = PS ? nt / p.ntc : 0;
+    const int n0 = (nt - ph * p.ntc) * BN;
+    const int oHt = PS ? p.oH : p.Hout, oWt = PS ? p.oW : p.Wout;  // the output tensor's height and width
+    // output coordinates of this thread's row rr (of two) of the tile: valid, flat pixel, residual pixel, spatial index in the sample
+    auto locate = [&](int rr, bool& valid, long long& pix, long long& rpix, long long& spi) {
+      const int row = wg * 64 + wq * 16 + (lane >> 2) + 8 * rr;  // pixel index inside the tile box
+      const int wl = row % p.tw;
+      const int hl = (row / p.tw) % p.th;
+      const int dl = row / (p.tw * p.th);
+      // pixel (gh, gw) of the grid the tiles walk; sub-pixel form: low-res pixel (gh, gw) of phase (pa, pb) -> output pixel
+      // (2 gh + pa, 2 gw + pb) of the [oH][oW] output
+      const int gw = twi * p.tw + wl, gh = thi * p.th + hl, od = tdi * p.td + dl;
+      valid = (row < rows_a) && gw < p.Wout && gh < p.Hout && od < p.Dout;
+      const int ow = PS ? 2 * gw + (ph & 1) : gw, oh = PS ? 2 * gh + (ph >> 1) : gh;
+      spi = ((long long)od * oHt + oh) * oWt + ow;
+      pix = (long long)n * p.Dout * oHt * oWt + spi;
+      rpix = p.residual ? (((long long)n * p.rD + od) * p.rH + (oh >> p.res_shift)) * p.rW + (ow >> p.res_shift) : 0;
+    };
+    if (ksplit == 1 && (lane & 3) == 0 && (p.residual || p.post_add)) {
+      // the residual / post-add rows are first read after this tile's main loop: pull them into L2 now
+      const int nb = (BN < p.Cout - n0 ? BN : p.Cout - n0) * 4;
+      for (int rr = 0; rr < 2; ++rr) {
+        bool valid;
+        long long pix, rpix, spi;
+        locate(rr, valid, pix, rpix, spi);
+        if (!valid) continue;
+        if (p.residual) {
+          const char* rp = (const char*)(p.residual + rpix * p.Cout + n0);
+          for (int b = 0; b < nb; b += 128) asm volatile("prefetch.global.L2 [%0];" ::"l"(rp + b));
+        }
+        if (p.post_add) {
+          const char* rp = (const char*)(p.post_add + spi * p.Cout + n0);
+          for (int b = 0; b < nb; b += 128) asm volatile("prefetch.global.L2 [%0];" ::"l"(rp + b));
+        }
+      }
+    }
+
+    // ---- fp32 register accumulation of the short wgmma chunks, starting from the bias (un-split layers) ----
+    if (p.bias && ksplit == 1) {
+      // fp16 operands: the sums are multiplied by out_scale (a power of two) below: exact
+      const float binv = F16 ? 1.f / p.out_scale : 1.f;
+#pragma unroll
+      for (int j = 0; j < kMaxBN / 8; ++j) {
+        const int c = n0 + 8 * j + cq;
+        float b0 = 0.f, b1 = 0.f;
+        if (8 * j < BN) {
+          if (c < p.Cout) b0 = __ldg(p.bias + c) * binv;
+          if (c + 1 < p.Cout) b1 = __ldg(p.bias + c + 1) * binv;
+        }
+        acc[4 * j] = b0; acc[4 * j + 1] = b1; acc[4 * j + 2] = b0; acc[4 * j + 3] = b1;
+      }
+    } else {
+#pragma unroll
+      for (int j = 0; j < kMaxBN / 2; ++j) acc[j] = 0.f;
+    }
+
+    uint64_t* pend_b = nullptr;
+    uint64_t* pend_a = nullptr;
+    // the main loop is instantiated per N tile width: the k-steps are then straight-line wgmma code of one shape
+    wgmma_dispatch_n(BN, [&](auto n_tile) {
+    if (p.yreuse) {
+      const int ngroups = p.kd * p.kw * p.kchunks;
+      const uint32_t row_shift = (uint32_t)p.tw * KC * 2;  // one image row of the halo tile: a whole number of swizzle atoms
+      int ks = 0;
+      for (int gi = 0; gi < ngroups; ++gi) {
+        mbar_wait(&afull_bar[sa], pha);
+        EMO_STAMP(4, et == 0 && item == tile_first && gi == 0);
+        for (int b = 0; b < p.kh; ++b, ++ks) {
+          const bool chunk_first = (ks % F) == 0;
+          const bool chunk_last = ((ks + 1) % F) == 0 || ks == nks - 1;
+          mbar_wait(&full_bar[sb], phb);
+          issue_kstep(n_tile, smem_u32(smem + (size_t)sa * a_halo_bytes) + (uint32_t)b * row_shift + wg_off, a_halo_plane,
+                      smem_u32(b_ring + (size_t)sb * b_tile_bytes), chunk_first);
+          // the halo tile is released with the last of its kh tap rows
+          finish_kstep(chunk_last, pend_b, pend_a, &empty_bar[sb], b == p.kh - 1 ? &aempty_bar[sa] : nullptr);
+          if (++sb == p.sb) { sb = 0; phb ^= 1; }
+        }
+        if (++sa == p.sa) { sa = 0; pha ^= 1; }
+      }
+    } else {
+      for (int ks = 0; ks < nks; ++ks) {
+        const bool chunk_first = (ks % F) == 0;
+        const bool chunk_last = ((ks + 1) % F) == 0 || ks == nks - 1;
+        mbar_wait(&full_bar[stage], phase);
+        EMO_STAMP(4, et == 0 && item == tile_first && ks == 0);
+        const uint32_t st = smem_u32(smem + (size_t)stage * stage_bytes);
+        issue_kstep(n_tile, st + wg_off, a_bytes, st + NP * a_bytes, chunk_first);
+        finish_kstep(chunk_last, pend_b, pend_a, &empty_bar[stage], nullptr);
+        if (++stage == S) { stage = 0; phase ^= 1; }
+      }
+    }
+    });
+    EMO_STAMP(5, et == 0);
+    if constexpr (F16) {
+      // the operand planes carried power-of-two scales (activations x sa, weights x sw): undo them on the fp32 sums (exact)
+#pragma unroll
+      for (int j = 0; j < kMaxBN / 2; ++j) acc[j] *= p.out_scale;
+    }
+
+    // ---- final phase: this thread's two rows ----
+    if (ksplit > 1) {
+      // split-K: this part's partial tile goes to ITS OWN slice of the fp32 workspace (plain stores: every output element
+      // is written exactly once per part); the finalize kernel sums the parts in part order - a fixed order, so the result
+      // does not depend on which CTA finished first - and applies bias / residual / activation / statistics
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        bool valid;
+        long long pix, rpix, spi;
+        locate(rr, valid, pix, rpix, spi);
+        if (!valid) continue;
+        float* wrow = p.ws + (size_t)part * (size_t)p.ws_part_elems + pix * p.Cout;
+#pragma unroll
+        for (int j = 0; j < kMaxBN / 8; ++j) {
+          const int c = n0 + 8 * j + cq;
+          if (8 * j < BN) {
+            if (c < p.Cout) wrow[c] = acc[4 * j + 2 * rr];
+            if (c + 1 < p.Cout) wrow[c + 1] = acc[4 * j + 2 * rr + 1];
+          }
+        }
+      }
+      continue;
+    }
+    const long long sp = (long long)p.Dout * oHt * oWt;
+    const bool pairs = (p.Cout & 1) == 0;  // c even, Cout even: both columns of a pair exist, 8-byte aligned
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) {
+      bool valid;
+      long long pix, rpix, spi;
+      locate(rr, valid, pix, rpix, spi);
+      // the row's residual / post-add values are loaded together before any store (a load may not move over a store that
+      // may alias it, so loads interleaved with the stores would each wait out a full memory latency); they are kept in the
+      // chunk registers, which are free until the next tile's main loop
+#pragma unroll
+      for (int j = 0; j < kMaxBN / 8; ++j) {
+        const int c = n0 + 8 * j + cq;
+        float2 r2 = make_float2(0.f, 0.f), p2 = make_float2(0.f, 0.f);
+        if (8 * j < BN && pairs && valid && c < p.Cout) {
+          if (p.residual) r2 = __ldg((const float2*)(p.residual + rpix * p.Cout + c));
+          if (p.post_add) p2 = __ldg((const float2*)(p.post_add + spi * p.Cout + c));
+        }
+        cf[2 * j] = r2.x; cf[2 * j + 1] = r2.y; cf[kMaxBN / 4 + 2 * j] = p2.x; cf[kMaxBN / 4 + 2 * j + 1] = p2.y;
+      }
+#pragma unroll
+      for (int j = 0; j < kMaxBN / 8; ++j) {
+        if (8 * j >= BN) continue;
+        const int c = n0 + 8 * j + cq;
+        float v0 = acc[4 * j + 2 * rr], v1 = acc[4 * j + 2 * rr + 1];
+        if (valid && c < p.Cout) {
+          if (pairs) {
+            v0 = act_apply(v0 + cf[2 * j], p.act) + cf[kMaxBN / 4 + 2 * j];
+            v1 = act_apply(v1 + cf[2 * j + 1], p.act) + cf[kMaxBN / 4 + 2 * j + 1];
+            if (!p.out_nchw) {
+              *(float2*)(p.out + pix * p.Cout + c) = make_float2(v0, v1);
+            } else {
+              p.out[((long long)n * p.Cout + c) * sp + spi] = v0;
+              p.out[((long long)n * p.Cout + c + 1) * sp + spi] = v1;
+            }
+          } else {
+            // odd channel count (e.g. Cout = 3): scalar path
+#pragma unroll
+            for (int q = 0; q < 2; ++q) {
+              const int cc = c + q;
+              float x = q ? v1 : v0;
+              if (cc < p.Cout) {
+                if (p.residual) x += __ldg(p.residual + rpix * p.Cout + cc);
+                x = act_apply(x, p.act);
+                if (p.post_add) x += __ldg(p.post_add + spi * p.Cout + cc);
+                if (!p.out_nchw) p.out[pix * p.Cout + cc] = x;
+                else p.out[((long long)n * p.Cout + cc) * sp + spi] = x;
+              } else {
+                x = 0.f;
+              }
+              if (q) v1 = x; else v0 = x;
+            }
+          }
+        } else {
+          v0 = 0.f; v1 = 0.f;  // pixels / channels outside the tensor: no part of the statistics
+        }
+        acc[4 * j + 2 * rr] = v0; acc[4 * j + 2 * rr + 1] = v1;
+      }
+    }
+    EMO_STAMP(6, et == 0);
+
+    if (p.stats) {
+      // column sums of the warp's 16 rows: two rows in the thread, then a butterfly over the eight lanes sharing the columns
+      float* cs = col_sum + warp * kMaxBN;
+      float* cqs = col_sq + warp * kMaxBN;
+#pragma unroll
+      for (int j = 0; j < kMaxBN / 8; ++j) {
+        if (8 * j >= BN) continue;
+        float s0 = acc[4 * j] + acc[4 * j + 2], s1 = acc[4 * j + 1] + acc[4 * j + 3];
+        float q0 = acc[4 * j] * acc[4 * j] + acc[4 * j + 2] * acc[4 * j + 2];
+        float q1 = acc[4 * j + 1] * acc[4 * j + 1] + acc[4 * j + 3] * acc[4 * j + 3];
+#pragma unroll
+        for (int off = 4; off < 32; off <<= 1) {
+          s0 += __shfl_xor_sync(0xffffffffu, s0, off);
+          s1 += __shfl_xor_sync(0xffffffffu, s1, off);
+          q0 += __shfl_xor_sync(0xffffffffu, q0, off);
+          q1 += __shfl_xor_sync(0xffffffffu, q1, off);
+        }
+        if (lane < 4) {
+          cs[8 * j + cq] = s0; cs[8 * j + cq + 1] = s1;
+          cqs[8 * j + cq] = q0; cqs[8 * j + cq + 1] = q1;
+        }
+      }
+      asm volatile("bar.sync 1, %0;" ::"n"(kConsumerWarps * 32) : "memory");
+      tile_group_stats(p, col_sum, col_sq, n, n0, BN, et, kConsumerWarps * 32);
+      asm volatile("bar.sync 1, %0;" ::"n"(kConsumerWarps * 32) : "memory");  // the slots are rewritten by the next tile
+    }
+    EMO_STAMP(7, et == 0);
+  }
+  EMO_STAMP(8, et == 0);
+}
 
 // split-K finalize: out = act(sum_parts ws[part] + bias + residual) + post_add, statistics.  The parts are summed in part
 // order (fixed), so the output is reproducible run to run.
@@ -451,6 +924,27 @@ static int pick_box(int dim, int want) {
   return b < 1 ? 1 : b;
 }
 
+// The kernel instantiations, indexed by EMO_CONV_KERNEL_*: plan_conv picks a row, emo_conv_igemm launches that row's kernel.
+struct ConvKernel {
+  int KC, NP;
+  bool ps, f16;
+  void (*fn)(TMaps, ConvKParams);
+};
+static const ConvKernel kConvKernels[] = {
+    {64, 2, false, false, conv_igemm_kernel<64, 2, false, false>},  // EMO_CONV_KERNEL_BF16X2_KC64
+    {32, 2, false, false, conv_igemm_kernel<32, 2, false, false>},  // EMO_CONV_KERNEL_BF16X2_KC32
+    {64, 3, false, false, conv_igemm_kernel<64, 3, false, false>},  // EMO_CONV_KERNEL_BF16X3_KC64
+    {32, 3, false, false, conv_igemm_kernel<32, 3, false, false>},  // EMO_CONV_KERNEL_BF16X3_KC32
+    {64, 2, false, true, conv_igemm_kernel<64, 2, false, true>},    // EMO_CONV_KERNEL_F16_KC64
+    {32, 2, false, true, conv_igemm_kernel<32, 2, false, true>},    // EMO_CONV_KERNEL_F16_KC32
+    {64, 2, true, false, conv_igemm_kernel<64, 2, true, false>},    // EMO_CONV_KERNEL_UPCONV_KC64
+    {64, 1, false, true, conv_igemm_kernel<64, 1, false, true>},    // EMO_CONV_KERNEL_H1_KC64
+    {32, 1, false, true, conv_igemm_kernel<32, 1, false, true>},    // EMO_CONV_KERNEL_H1_KC32
+    {64, 1, true, true, conv_igemm_kernel<64, 1, true, true>},      // EMO_CONV_KERNEL_H1_UPCONV_KC64
+};
+static constexpr int kNumConvKernels = (int)(sizeof(kConvKernels) / sizeof(kConvKernels[0]));
+static_assert(kNumConvKernels == EMO_CONV_KERNEL_H1_UPCONV_KC64 + 1, "one row per EMO_CONV_KERNEL_* id");
+
 // What emo_conv_igemm runs for one descriptor: the kernel parameters (tiles, N tile, k-chunk, pipeline depths, split-K,
 // accumulation chunk), the kernel form, the grid, the shared-memory size and the launches that finish the convolution.
 struct ConvPlan {
@@ -631,11 +1125,12 @@ static int plan_conv(const emo_conv_desc* d, int sm_count, ConvPlan* plan) {
   else
     plan->finish = post ? EMO_CONV_FINISH_APPLY : EMO_CONV_FINISH_NONE;
   plan->NP = NP; plan->KC = KC; plan->f16 = f16; plan->ps = ps; plan->kh_eff = kh_eff;
-  plan->kernel = NP == 1 ? (ps ? EMO_CONV_KERNEL_H1_UPCONV_KC64 : KC == 64 ? EMO_CONV_KERNEL_H1_KC64 : EMO_CONV_KERNEL_H1_KC32)
-                 : f16 ? (KC == 64 ? EMO_CONV_KERNEL_F16_KC64 : EMO_CONV_KERNEL_F16_KC32)
-                 : ps ? EMO_CONV_KERNEL_UPCONV_KC64
-                 : NP == 3 ? (KC == 64 ? EMO_CONV_KERNEL_BF16X3_KC64 : EMO_CONV_KERNEL_BF16X3_KC32)
-                           : (KC == 64 ? EMO_CONV_KERNEL_BF16X2_KC64 : EMO_CONV_KERNEL_BF16X2_KC32);
+  plan->kernel = -1;
+  for (int k = 0; k < kNumConvKernels; ++k) {
+    const ConvKernel& r = kConvKernels[k];
+    if (r.NP == NP && r.f16 == (f16 != 0) && r.ps == (ps != 0) && r.KC == KC) plan->kernel = k;
+  }
+  EMO_REQUIRE(plan->kernel >= 0, "emo_conv_igemm: internal error: no kernel for NP=%d fp16=%d upconv=%d KC=%d", NP, f16, ps, KC);
   plan->grid = grid;
   plan->smem_bytes = smem_bytes;
   return EMO_OK;
@@ -717,37 +1212,17 @@ extern "C" int emo_conv_igemm(const emo_conv_desc* d, void* stream_) {
     }
   }
 
+  const auto kernel = kConvKernels[plan.kernel].fn;
+  static bool attr_set[kNumConvKernels][64] = {};  // the opt-in is per function AND per device (227 KB covers every configuration)
   cudaError_t e;
-#define EMO_LAUNCH_CONV(KERNEL_, KC_, NP_)                                                                                 \
-  do {                                                                                                                    \
-    static bool attr_set_dev[64] = {false}; /* the opt-in is per function AND per device (227 KB covers every configuration) */ \
-    bool& attr_set = attr_set_dev[cur_dev & 63];                                                                          \
-    if (!attr_set) {                                                                                                      \
-      e = cudaFuncSetAttribute(KERNEL_<KC_, NP_>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);               \
-      if (e != cudaSuccess) { set_error("emo_conv_igemm: smem attribute: %s", cudaGetErrorString(e)); return EMO_ERR_CUDA; } \
-      attr_set = true;                                                                                                    \
-    }                                                                                                                     \
-    KERNEL_<KC_, NP_><<<grid, kThreads, smem_bytes, stream>>>(tm, p);                                                     \
-    e = cudaGetLastError();                                                                                               \
-    if (e != cudaSuccess) { set_error("emo_conv_igemm: launch: %s", cudaGetErrorString(e)); return EMO_ERR_CUDA; }         \
-  } while (0)
-  if (NP == 1) {
-    if (ps) EMO_LAUNCH_CONV(conv_igemm_ps_f16_kernel, 64, 1);
-    else if (KC == 64) EMO_LAUNCH_CONV(conv_igemm_f16_kernel, 64, 1);
-    else EMO_LAUNCH_CONV(conv_igemm_f16_kernel, 32, 1);
-  } else if (f16) {
-    if (KC == 64) EMO_LAUNCH_CONV(conv_igemm_f16_kernel, 64, 2);
-    else EMO_LAUNCH_CONV(conv_igemm_f16_kernel, 32, 2);
-  } else if (ps) {
-    EMO_LAUNCH_CONV(conv_igemm_ps_kernel, 64, 2);
-  } else if (NP == 3) {
-    if (KC == 64) EMO_LAUNCH_CONV(conv_igemm_kernel, 64, 3);
-    else EMO_LAUNCH_CONV(conv_igemm_kernel, 32, 3);
-  } else {
-    if (KC == 64) EMO_LAUNCH_CONV(conv_igemm_kernel, 64, 2);
-    else EMO_LAUNCH_CONV(conv_igemm_kernel, 32, 2);
+  if (!attr_set[plan.kernel][cur_dev & 63]) {
+    e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    if (e != cudaSuccess) { set_error("emo_conv_igemm: smem attribute: %s", cudaGetErrorString(e)); return EMO_ERR_CUDA; }
+    attr_set[plan.kernel][cur_dev & 63] = true;
   }
-#undef EMO_LAUNCH_CONV
+  kernel<<<grid, kThreads, smem_bytes, stream>>>(tm, p);
+  e = cudaGetLastError();
+  if (e != cudaSuccess) { set_error("emo_conv_igemm: launch: %s", cudaGetErrorString(e)); return EMO_ERR_CUDA; }
   const emo_apply_desc* post = d->post;
   if (plan.finish == EMO_CONV_FINISH_POST) {
     // small split-K layer with a post-op: one cluster per sample finishes the convolution, normalises, activates and writes the

@@ -81,16 +81,131 @@ __global__ void gn_finalize_kernel(const emo_gn_finalize_desc d) {
 #ifndef EMO_APPLY_MIN_CTAS
 #define EMO_APPLY_MIN_CTAS 4
 #endif
-#define EMO_APPLY_F16 0
-#define EMO_APPLY_KERNEL_NAME apply_kernel
-#include "apply_kernel.inc"
-#undef EMO_APPLY_F16
-#undef EMO_APPLY_KERNEL_NAME
-#define EMO_APPLY_F16 1
-#define EMO_APPLY_KERNEL_NAME apply_f16_kernel
-#include "apply_kernel.inc"
-#undef EMO_APPLY_F16
-#undef EMO_APPLY_KERNEL_NAME
+// ---- apply: y = act(x*A + B [+ res*A2 + B2]) -> fp32 / 16-bit planes, optional nearest x2 on H,W ----
+// F16 = false: bf16 (hi, lo[, lo2]) planes of y; F16 = true: fp16 planes of y * plane_scale for the fp16 operand modes of the
+// convolution (hi alone when out_lo is NULL).
+// __launch_bounds__(256, EMO_APPLY_MIN_CTAS = 4): 64 registers, 4 resident CTAs per SM (the unconstrained build took 66 registers ->
+// 3 CTAs; measured round 2: +1% on the whole frame, no spills; 6 CTAs with spills is slower, see above).  ReLU / no activation is a
+// branch-free max (the general act_apply switch is a jump table per element): 58.9 -> 56.1 us at 512^2 x 128.
+// V = float4s per thread (2 when C % 8 == 0: 32 B loads, 16-byte plane stores)
+template <int UP, int V, bool F16>
+__global__ void __launch_bounds__(256, EMO_APPLY_MIN_CTAS) apply_kernel(const emo_apply_desc d) {
+  extern __shared__ float sAB[];  // fused finalisation: A[C] then B[C] of this CTA's sample
+  const int cvn = d.C / (4 * V);  // channel-vector slots per position
+  const long long S = (long long)d.D * d.H * d.W;
+  const int n = blockIdx.y;
+  if (d.stats) {
+    const int cpg = d.C / d.G;
+    for (int c = threadIdx.x; c < d.C; c += blockDim.x) {
+      const int g = c / cpg;
+      const double s = d.stats[((long long)n * d.G + g) * 2], q = d.stats[((long long)n * d.G + g) * 2 + 1];
+      const double mean = s / d.count;
+      double var = q / d.count - mean * mean;
+      if (var < 0) var = 0;
+      const float rstd = (float)(1.0 / sqrt(var + (double)d.eps));
+      float gam = d.gamma ? d.gamma[c] : 1.f, bet = d.beta ? d.beta[c] : 0.f;
+      if (d.ada_w) {
+        const float aw = d.ada_w[(long long)n * d.C + c], ab = d.ada_b[(long long)n * d.C + c];
+        bet = bet * aw + ab;
+        gam = gam * aw;
+      }
+      const float A = rstd * gam;
+      sAB[c] = A;
+      sAB[d.C + c] = bet - (float)mean * A;
+    }
+    __syncthreads();
+  }
+  const long long per_n = S * cvn;
+  const bool simple_act = d.act == EMO_ACT_RELU || d.act == EMO_ACT_NONE;
+  const float act_lo = d.act == EMO_ACT_RELU ? 0.f : -INFINITY;
+  const float4* x4 = (const float4*)d.x + (long long)n * per_n * V;
+  const float4* r4 = d.res ? (const float4*)d.res + (long long)n * per_n * V : nullptr;
+  const float* gA = d.A ? d.A + (d.ab_per_sample ? (long long)n * d.C : 0) : nullptr;
+  const float* gB = d.B ? d.B + (d.ab_per_sample ? (long long)n * d.C : 0) : nullptr;
+  // channel-vector slot of this thread: one 64-bit modulo up front, then stepped with the (uniform) grid stride - the 64-bit
+  // `tt % cvn` per iteration was ~80 of the ~250 instructions of an iteration (emulated division)
+  const long long tt0 = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long long tstride = (long long)gridDim.x * blockDim.x;
+  int cv = (int)(tt0 % cvn);
+  const int cv_step = (int)(tstride % cvn);
+  for (long long tt = tt0; tt < per_n; tt += tstride, cv = (cv + cv_step >= cvn) ? cv + cv_step - cvn : cv + cv_step) {
+    float4 v[V];
+#pragma unroll
+    for (int u = 0; u < V; ++u) v[u] = __ldg(x4 + tt * V + u);
+#pragma unroll
+    for (int u = 0; u < V; ++u) {
+      const int c = (cv * V + u) * 4;
+      if (d.stats) {
+        const float4 a = *(const float4*)&sAB[c];
+        const float4 b = *(const float4*)&sAB[d.C + c];
+        v[u].x = fmaf(v[u].x, a.x, b.x); v[u].y = fmaf(v[u].y, a.y, b.y); v[u].z = fmaf(v[u].z, a.z, b.z); v[u].w = fmaf(v[u].w, a.w, b.w);
+      } else if (gA) {
+        const float4 a = __ldg((const float4*)(gA + c));
+        const float4 b = __ldg((const float4*)(gB + c));
+        v[u].x = fmaf(v[u].x, a.x, b.x); v[u].y = fmaf(v[u].y, a.y, b.y); v[u].z = fmaf(v[u].z, a.z, b.z); v[u].w = fmaf(v[u].w, a.w, b.w);
+      }
+      if (r4) {
+        float4 r = __ldg(r4 + tt * V + u);
+        if (d.A2) {
+          const float4 a = __ldg((const float4*)(d.A2 + c));
+          const float4 b = __ldg((const float4*)(d.B2 + c));
+          r.x = fmaf(r.x, a.x, b.x); r.y = fmaf(r.y, a.y, b.y); r.z = fmaf(r.z, a.z, b.z); r.w = fmaf(r.w, a.w, b.w);
+        }
+        v[u].x += r.x; v[u].y += r.y; v[u].z += r.z; v[u].w += r.w;
+      }
+      if (simple_act) {  // ReLU / none: one branch-free max (act_apply's switch compiles to a jump table per element)
+        v[u].x = fmaxf(v[u].x, act_lo); v[u].y = fmaxf(v[u].y, act_lo); v[u].z = fmaxf(v[u].z, act_lo); v[u].w = fmaxf(v[u].w, act_lo);
+      } else {
+        v[u].x = act_apply(v[u].x, d.act); v[u].y = act_apply(v[u].y, d.act);
+        v[u].z = act_apply(v[u].z, d.act); v[u].w = act_apply(v[u].w, d.act);
+      }
+    }
+    uint2 hi[V], lo[V], lo2[V];
+    if (d.out_hi) {
+#pragma unroll
+      for (int u = 0; u < V; ++u) {
+        if constexpr (F16) {
+          split4_h(v[u], d.plane_scale, hi[u], lo[u]);  // fp16 planes of y * plane_scale (hi alone when out_lo is NULL)
+          lo2[u] = make_uint2(0u, 0u);
+        } else {
+          if (d.out_lo2) split4x3(v[u], hi[u], lo[u], lo2[u]);
+          else split4(v[u], hi[u], lo[u]);
+        }
+      }
+    }
+    auto store = [&](long long o) {  // o = float4-slot index of the first vector of this thread in the output tensor
+      if (d.out) {
+#pragma unroll
+        for (int u = 0; u < V; ++u) ((float4*)d.out)[o + u] = v[u];
+      }
+      if (d.out_hi) {
+        if (V == 2) {
+          ((uint4*)d.out_hi)[o >> 1] = make_uint4(hi[0].x, hi[0].y, hi[V - 1].x, hi[V - 1].y);
+          if (!F16 || d.out_lo) ((uint4*)d.out_lo)[o >> 1] = make_uint4(lo[0].x, lo[0].y, lo[V - 1].x, lo[V - 1].y);
+          if (d.out_lo2) ((uint4*)d.out_lo2)[o >> 1] = make_uint4(lo2[0].x, lo2[0].y, lo2[V - 1].x, lo2[V - 1].y);
+        } else {
+          ((uint2*)d.out_hi)[o] = hi[0];
+          if (!F16 || d.out_lo) ((uint2*)d.out_lo)[o] = lo[0];
+          if (d.out_lo2) ((uint2*)d.out_lo2)[o] = lo2[0];
+        }
+      }
+    };
+    if (UP == 1) {
+      store(((long long)n * per_n + tt) * V);
+    } else {
+      const long long s = tt / cvn;  // spatial position inside the sample
+      const int w = (int)(s % d.W);
+      const int h = (int)((s / d.W) % d.H);
+      const int dd = (int)(s / ((long long)d.W * d.H));
+      const int H2 = d.H * UP, W2 = d.W * UP;
+#pragma unroll
+      for (int uy = 0; uy < UP; ++uy)
+#pragma unroll
+        for (int ux = 0; ux < UP; ++ux)
+          store((((((long long)n * d.D + dd) * H2 + (h * UP + uy)) * W2 + (w * UP + ux)) * cvn + cv) * V);
+    }
+  }
+}
 
 // Image head (emo_gn_head): one warp handles 8 pixels per step.  Lane l owns channels 4l..4l+3 (+128k): a warp load reads a
 // pixel's whole channel vector (512 B at C = 128); the 8 x 4 per-lane partial dot products are transpose-reduced over the
@@ -252,18 +367,12 @@ extern "C" int emo_apply(const emo_apply_desc* d, void* stream_) {
   const dim3 grid((unsigned)blocks, (unsigned)d->N);
   const size_t smem = d->stats ? 2 * (size_t)d->C * sizeof(float) : 0;
   EMO_REQUIRE(smem <= 48 * 1024, "emo_apply: C=%d too large for the fused finalisation", d->C);
-  if (d->plane_fp16) {
+  if (d->plane_fp16)
     EMO_REQUIRE(!d->out_lo2 && d->plane_scale > 0.f, "emo_apply: fp16 planes are one or two (no out_lo2) and need a positive plane_scale");
-    if (d->up == 1 && V == 2) launch_kernel(apply_f16_kernel<1, 2>, grid, 256, smem, stream, *d);
-    else if (d->up == 1) launch_kernel(apply_f16_kernel<1, 1>, grid, 256, smem, stream, *d);
-    else if (V == 2) launch_kernel(apply_f16_kernel<2, 2>, grid, 256, smem, stream, *d);
-    else launch_kernel(apply_f16_kernel<2, 1>, grid, 256, smem, stream, *d);
-    return check_launch("emo_apply");
-  }
-  if (d->up == 1 && V == 2) launch_kernel(apply_kernel<1, 2>, grid, 256, smem, stream, *d);
-  else if (d->up == 1) launch_kernel(apply_kernel<1, 1>, grid, 256, smem, stream, *d);
-  else if (V == 2) launch_kernel(apply_kernel<2, 2>, grid, 256, smem, stream, *d);
-  else launch_kernel(apply_kernel<2, 1>, grid, 256, smem, stream, *d);
+  static void (*const kernels[2][2][2])(emo_apply_desc) = {  // [fp16 planes][up - 1][V - 1]
+      {{apply_kernel<1, 1, false>, apply_kernel<1, 2, false>}, {apply_kernel<2, 1, false>, apply_kernel<2, 2, false>}},
+      {{apply_kernel<1, 1, true>, apply_kernel<1, 2, true>}, {apply_kernel<2, 1, true>, apply_kernel<2, 2, true>}}};
+  launch_kernel(kernels[d->plane_fp16 ? 1 : 0][d->up - 1][V - 1], grid, 256, smem, stream, *d);
   return check_launch("emo_apply");
 }
 

@@ -162,6 +162,13 @@ __device__ __forceinline__ void wgmma_f16(float* d, uint64_t da, uint64_t db, ui
   else if constexpr (N == 128) wgmma_f16_n128(d, da, db, scale_d);
 }
 
+// fp16 (F16) or bf16 operands
+template <bool F16, int N>
+__device__ __forceinline__ void wgmma(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
+  if constexpr (F16) wgmma_f16<N>(d, da, db, scale_d);
+  else wgmma_bf16<N>(d, da, db, scale_d);
+}
+
 // Runs f(std::integral_constant<int, N>) for the N tile chosen at run time (uniform across the CTA): the wgmmas of one
 // k-step are then straight-line code for one instruction shape.
 template <class F>

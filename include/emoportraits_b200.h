@@ -249,17 +249,18 @@ int emo_conv_igemm(const emo_conv_desc* d, void* stream);
  * call, no device needed, pointers are checked (null, alignment) but never dereferenced.  Runs the same argument checks
  * and returns the same error codes as emo_conv_igemm. */
 enum {
-  EMO_CONV_KERNEL_BF16X2_KC64 = 0, /* conv_igemm_kernel<64, 2> */
-  EMO_CONV_KERNEL_BF16X2_KC32 = 1, /* conv_igemm_kernel<32, 2> */
-  EMO_CONV_KERNEL_BF16X3_KC64 = 2, /* conv_igemm_kernel<64, 3> */
-  EMO_CONV_KERNEL_BF16X3_KC32 = 3, /* conv_igemm_kernel<32, 3> */
-  EMO_CONV_KERNEL_F16_KC64 = 4,    /* conv_igemm_f16_kernel<64, 2> */
-  EMO_CONV_KERNEL_F16_KC32 = 5,    /* conv_igemm_f16_kernel<32, 2> */
-  EMO_CONV_KERNEL_UPCONV_KC64 = 6, /* conv_igemm_ps_kernel<64, 2> */
+  /* conv_igemm_kernel<KC, NP, PS (sub-pixel form), F16 (fp16 operands)> */
+  EMO_CONV_KERNEL_BF16X2_KC64 = 0, /* conv_igemm_kernel<64, 2, false, false> */
+  EMO_CONV_KERNEL_BF16X2_KC32 = 1, /* conv_igemm_kernel<32, 2, false, false> */
+  EMO_CONV_KERNEL_BF16X3_KC64 = 2, /* conv_igemm_kernel<64, 3, false, false> */
+  EMO_CONV_KERNEL_BF16X3_KC32 = 3, /* conv_igemm_kernel<32, 3, false, false> */
+  EMO_CONV_KERNEL_F16_KC64 = 4,    /* conv_igemm_kernel<64, 2, false, true> */
+  EMO_CONV_KERNEL_F16_KC32 = 5,    /* conv_igemm_kernel<32, 2, false, true> */
+  EMO_CONV_KERNEL_UPCONV_KC64 = 6, /* conv_igemm_kernel<64, 2, true, false> */
   /* one-plane fp16 operands (operand_fp16 with a_lo == w_lo == NULL), reported with NP = 1; ids 7, 8, 9 */
-  EMO_CONV_KERNEL_H1_KC64,         /* conv_igemm_f16_kernel<64, 1> */
-  EMO_CONV_KERNEL_H1_KC32,         /* conv_igemm_f16_kernel<32, 1> */
-  EMO_CONV_KERNEL_H1_UPCONV_KC64   /* conv_igemm_ps_f16_kernel<64, 1> */
+  EMO_CONV_KERNEL_H1_KC64,         /* conv_igemm_kernel<64, 1, false, true> */
+  EMO_CONV_KERNEL_H1_KC32,         /* conv_igemm_kernel<32, 1, false, true> */
+  EMO_CONV_KERNEL_H1_UPCONV_KC64   /* conv_igemm_kernel<64, 1, true, true> */
 };
 enum {
   EMO_CONV_FINISH_NONE = 0,           /* the convolution kernel writes the output */

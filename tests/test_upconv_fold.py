@@ -1,6 +1,6 @@
 """CPU tests of the sub-pixel form of `nearest x2 -> 3x3 conv` (emo_conv_desc.upconv, ops.fold_upconv_weight):
-the weight folding is exact algebra, and the index arithmetic the CUDA kernel uses (conv_igemm_kernel.inc, EMO_CONV_PS
-blocks: tile origin - pad + phase shift + tap, weight row phase * 4 + tap, output pixel 2 g + parity) is restated here
+the weight folding is exact algebra, and the index arithmetic the CUDA kernel uses (conv_igemm.cu, conv_igemm_kernel with
+PS = true: tile origin - pad + phase shift + tap, weight row phase * 4 + tap, output pixel 2 g + parity) is restated here
 with torch gathers and compared with F.conv2d on the upsampled map."""
 import torch
 import torch.nn.functional as F
@@ -81,7 +81,7 @@ def _pick_box(dim, want):
 
 
 def test_subpixel_tile_walk_restated():
-    """Host parameters (emo_conv_igemm, upconv branch) and device index logic (conv_igemm_kernel.inc, EMO_CONV_PS blocks)
+    """Host parameters (emo_conv_igemm, upconv branch) and device index logic (conv_igemm_kernel with PS = true)
     restated for a multi-tile case: 128-pixel boxes over the low-res grid, N tile = (phase, channel tile), TMA box gather
     with zero fill, pixel-shuffle store.  Every output element must be written exactly once with the reference value."""
     from emoportraits_b200.ops import fold_upconv_weight

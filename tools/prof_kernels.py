@@ -1,8 +1,9 @@
 """Representative launches of every roofline kernel for `ncu --set full` captures, e.g.
    ncu --set full -k regex:conv_igemm -o conv python tools/prof_kernels.py
    conv_igemm_kernel   decoder 3x3 512->512 @64^2 with residual (dominant layer), 3x3 128->128 @512^2 with
-                       residual (row-reuse main loop), sub-pixel up-conv 192->128 @256^2 -> 512^2
-   conv_igemm_f16_kernel  warp-generator 3x3x3 64->32 @32x64x64 (fp16 two-plane operands), ResNet-18 3x3 64->64 @32^2 (split-K)
+                       residual (row-reuse main loop), sub-pixel up-conv 192->128 @256^2 -> 512^2 (PS = true);
+                       F16 = true: warp-generator 3x3x3 64->32 @32x64x64 (fp16 two-plane operands), ResNet-18 3x3 64->64
+                       @32^2 (split-K)
    splitk_post_kernel  the fused finalize + GroupNorm + ReLU + plane split behind that split-K layer
    apply_kernel        GroupNorm-apply + ReLU + plane split @512^2 x 128
    gn_head_kernel      image head @512^2 x 128 -> 3
