@@ -42,23 +42,36 @@ class ConvW:
 
 
 class Norm:
+    """GroupNorm(32), or eval-mode BatchNorm (recognised by its `running_mean`) folded to the per-channel y = x*A + B."""
+
     def __init__(self, sd, p, dev):
         self.gamma = sd[p + ".weight"].detach().float().to(dev).contiguous()
         self.beta = sd[p + ".bias"].detach().float().to(dev).contiguous()
-        self.C = self.gamma.numel()
-        self.gb = torch.stack([self.gamma, self.beta]).contiguous()  # (2, C): `add` operand of the projector GEMM
+        self.needs_stats = (p + ".running_mean") not in sd
+        if not self.needs_stats:
+            g, b = sd[p + ".weight"].float(), sd[p + ".bias"].float()
+            m, v = sd[p + ".running_mean"].float(), sd[p + ".running_var"].float()
+            A = g / torch.sqrt(v + 1e-5)
+            self.A = A[None].to(dev).contiguous()
+            self.B = (b - m * A)[None].to(dev).contiguous()
 
-    def affine(self, stats, count, ada=None):
-        if ada is None:
-            return ops.gn_finalize(stats, count, self.gamma, self.beta)
-        return ops.gn_finalize(stats, count, self.gamma, self.beta, ada_w=ada[0], ada_b=ada[1])
+    def affine(self, stats, count):
+        if not self.needs_stats:
+            return self.A, self.B
+        return ops.gn_finalize(stats, count, self.gamma, self.beta)
 
     def gn(self, stats, count, ada=None):
-        """arguments of the finalisation fused into ops.apply"""
+        """arguments of the GroupNorm finalisation fused into ops.apply"""
         d = dict(stats=stats, count=count, gamma=self.gamma, beta=self.beta)
         if ada is not None:
             d.update(ada_w=ada[0], ada_b=ada[1])
         return d
+
+    def apply_args(self, stats=None, count=None, ada=None):
+        """keyword arguments of ops.apply (or of a conv `post=`) that normalise a tensor whose statistics are `stats`"""
+        if not self.needs_stats:
+            return dict(A=self.A, B=self.B, per_sample=False)
+        return dict(gn=self.gn(stats, count, ada))
 
 
 def _count(x):
@@ -66,8 +79,17 @@ def _count(x):
     return x.numel() / x.shape[0] / G
 
 
+def stem_weight(sd, p, dev):
+    """7x7 RGB stem conv -> ops.conv_direct operands: weight (7, 7, 4, Cout) with a zero 4th input channel, bias"""
+    w, b = fold_conv(sd, p)
+    wc = torch.zeros(7, 7, 4, w.shape[0])
+    wc[:, :, :3] = w.permute(2, 3, 1, 0)
+    return wc.to(dev).contiguous(), (b.to(dev).contiguous() if b is not None else None)
+
+
 class ResBlock:
-    """utils.py:661-788: [nearest up] -> norm -> relu -> conv -> norm -> relu -> conv [-> avgpool]; skip = [up] -> [1x1] -> [pool]."""
+    """utils.py:661-788: [nearest up] -> norm -> relu -> conv -> norm -> relu -> conv [-> avgpool]; skip = [up] -> [1x1] -> [pool].
+    The norms are GroupNorm (stage 1) or eval-mode BatchNorm (stage 2); only GroupNorm needs statistics."""
 
     def __init__(self, sd, p, dev, ws_first=True, planes=2, subpixel_up=False, pool_fold=False):
         self.planes = planes
@@ -94,25 +116,27 @@ class ResBlock:
             if tuple(w.shape[2:]) == (3, 3):
                 self.c2_pool = ops.pack_conv_weight(ops.fold_poolconv_weight(w), device=dev, planes=planes)
 
-    def __call__(self, x, sx, up=1, down=None, ada=None, want_stats=True):
+    def __call__(self, x, sx=None, up=1, down=None, ada=None, want_stats=True):
+        """x and its statistics sx (None for BatchNorm) -> (out, statistics of out: None for BatchNorm or want_stats=False)"""
         dev = x.device
         N = x.shape[0]
-        st1 = ops.new_stats(N, G, dev)
-        if up == 2 and self.c1_ps is not None and x.shape[1] == 1 and (x.shape[2] * x.shape[3]) % 256 == 0:
-            a = ops.apply(x, gn=self.n1.gn(sx, _count(x), ada[0] if ada else None), act=ops.ACT_RELU, up=1, planes=self.planes)
+        st1 = ops.new_stats(N, G, dev) if self.n2.needs_stats else None
+        subpixel = up == 2 and self.c1_ps is not None and x.shape[1] == 1 and (x.shape[2] * x.shape[3]) % 256 == 0
+        a = ops.apply(x, **self.n1.apply_args(sx, _count(x), ada[0] if ada else None), act=ops.ACT_RELU, up=1 if subpixel else up,
+                      planes=self.planes)
+        if subpixel:
             y = ops.conv_igemm(a, self.c1_ps, bias=self.c1.b, stats=st1, upconv=True)
-            b = ops.apply(y, gn=self.n2.gn(st1, _count(y), ada[1] if ada else None), act=ops.ACT_RELU, planes=self.planes)
+            b = ops.apply(y, **self.n2.apply_args(st1, _count(y), ada[1] if ada else None), act=ops.ACT_RELU, planes=self.planes)
         else:
-            a = ops.apply(x, gn=self.n1.gn(sx, _count(x), ada[0] if ada else None), act=ops.ACT_RELU, up=up, planes=self.planes)
             # conv -> norm -> relu: the second norm's pass is the convolution's post-op (one launch for the small split-K layers)
             cnt = a.shape[1] * a.shape[2] * a.shape[3] * self.c1.cout / G
             b = ops.conv_igemm(a, self.c1.w, bias=self.c1.b, stats=st1,
-                               post=dict(gn=self.n2.gn(st1, cnt, ada[1] if ada else None), act=ops.ACT_RELU, planes=self.planes))
+                               post=dict(**self.n2.apply_args(st1, cnt, ada[1] if ada else None), act=ops.ACT_RELU, planes=self.planes))
         # skip path: the 1x1 conv commutes with nearest-upsampling and with average pooling, so it runs at the smaller size
         s = ops.avgpool(x, down) if down else x
         if self.skip is not None:
             s = ops.conv_igemm(ops.split_bf16(s, self.planes), self.skip.w, bias=self.skip.b)
-        st2 = ops.new_stats(N, G, dev) if want_stats else None
+        st2 = ops.new_stats(N, G, dev) if (want_stats and self.n2.needs_stats) else None
         if down and self.c2_pool is not None and tuple(down) == (1, 2, 2) and b.shape[2] % 2 == 0 and b.shape[3] % 2 == 0:
             out = ops.conv_igemm(b, self.c2_pool, stride=(1, 2, 2), pad=(0, 1, 1), bias=self.c2.b, residual=s, stats=st2)
         elif down:
@@ -129,10 +153,7 @@ class LocalEncoder:
         self.planes = planes
         p = "local_encoder_nw"
         s = cfg.image_size
-        w, b = fold_conv(sd, f"{p}.from_rgb_{s}px")
-        wc = torch.zeros(7, 7, 4, w.shape[0])
-        wc[:, :, :3] = w.permute(2, 3, 1, 0)
-        self.stem_w, self.stem_b = wc.to(dev).contiguous(), b.to(dev).contiguous()
+        self.stem_w, self.stem_b = stem_weight(sd, f"{p}.from_rgb_{s}px", dev)
         self.blocks = []
         for i in range(len(cfg.enc_channels) - 1):
             self.blocks.append(ResBlock(sd, f"{p}.enc_{i}_block={s}px", dev, planes=planes, pool_fold=True))
@@ -159,38 +180,15 @@ class LocalEncoder:
 
 
 # ------------------------------------------------------------------------------------------------------------------
-class _RNNorm:
-    """ResNet norm: GroupNorm(32) (replace_bn_to_gn, utils.py:1020) or eval-mode BatchNorm folded to an affine."""
-
-    def __init__(self, sd, p, dev):
-        self.is_bn = (p + ".running_mean") in sd
-        if self.is_bn:
-            g, b = sd[p + ".weight"].float(), sd[p + ".bias"].float()
-            m, v = sd[p + ".running_mean"].float(), sd[p + ".running_var"].float()
-            A = g / torch.sqrt(v + 1e-5)
-            self.A = A[None].to(dev).contiguous()
-            self.B = (b - m * A)[None].to(dev).contiguous()
-        else:
-            self.n = Norm(sd, p, dev)
-
-    def affine(self, stats, count):
-        if self.is_bn:
-            return self.A, self.B
-        return self.n.affine(stats, count)
-
-
 class ResNet:
-    """torchvision resnet18 / resnet50 trunk (conv1..layer4) on channels-last tensors."""
+    """torchvision resnet18 / resnet50 trunk (conv1..layer4) on channels-last tensors; the norms are eval-mode BatchNorm or
+    GroupNorm(32) (replace_bn_to_gn, utils.py:1020)."""
 
     def __init__(self, sd, p, dev, gn: bool, planes=2):
         self.gn = gn
         self.planes = planes
-        w, b = fold_conv(sd, p + ".conv1")
-        wc = torch.zeros(7, 7, 4, w.shape[0])
-        wc[:, :, :3] = w.permute(2, 3, 1, 0)
-        self.stem_w = wc.to(dev).contiguous()
-        self.stem_b = b.to(dev).contiguous() if b is not None else None
-        self.bn1 = _RNNorm(sd, p + ".bn1", dev)
+        self.stem_w, self.stem_b = stem_weight(sd, p + ".conv1", dev)
+        self.bn1 = Norm(sd, p + ".bn1", dev)
         self.blocks = []
         for li in range(1, 5):
             bi = 0
@@ -198,15 +196,15 @@ class ResNet:
                 q = f"{p}.layer{li}.{bi}"
                 blk = dict(stride=2 if (li > 1 and bi == 0) else 1, bottleneck=(q + ".bn3.weight") in sd)
                 blk["c1"] = ConvW(sd, q + ".conv1", dev, planes=planes)
-                blk["n1"] = _RNNorm(sd, q + ".bn1", dev)
+                blk["n1"] = Norm(sd, q + ".bn1", dev)
                 blk["c2"] = ConvW(sd, q + ".conv2", dev, ws=gn, planes=planes)
-                blk["n2"] = _RNNorm(sd, q + ".bn2", dev)
+                blk["n2"] = Norm(sd, q + ".bn2", dev)
                 if blk["bottleneck"]:
                     blk["c3"] = ConvW(sd, q + ".conv3", dev, ws=gn, planes=planes)
-                    blk["n3"] = _RNNorm(sd, q + ".bn3", dev)
+                    blk["n3"] = Norm(sd, q + ".bn3", dev)
                 if (q + ".downsample.1.weight") in sd:
                     blk["cd"] = ConvW(sd, q + ".downsample.0", dev, planes=planes)
-                    blk["nd"] = _RNNorm(sd, q + ".downsample.1", dev)
+                    blk["nd"] = Norm(sd, q + ".downsample.1", dev)
                 self.blocks.append(blk)
                 bi += 1
 
@@ -221,27 +219,18 @@ class ResNet:
         a per-channel affine; GroupNorm is finalised from the convolution's own statistics."""
         kw.setdefault("planes", self.planes)
         N, _, Hi, Wi, _ = a.shape
-        if norm.is_bn:
-            return ops.conv_igemm(a, cw.w, stride=(1, stride, stride), bias=cw.b, post=dict(A=norm.A, B=norm.B, per_sample=False, **kw))
-        st = ops.new_stats(N, G, a.hi.device)
+        st = ops.new_stats(N, G, a.hi.device) if norm.needs_stats else None
         k = cw.w.k[1]
         Ho, Wo = (Hi + 2 * (k // 2) - k) // stride + 1, (Wi + 2 * (k // 2) - k) // stride + 1
         return ops.conv_igemm(a, cw.w, stride=(1, stride, stride), bias=cw.b, stats=st,
-                              post=dict(gn=norm.n.gn(st, Ho * Wo * cw.cout / G), **kw))
-
-    @staticmethod
-    def _napply(norm, y, st, **kw):
-        """norm + activation pass: eval-BatchNorm is a per-channel affine; GroupNorm is finalised inside the apply kernel"""
-        if norm.is_bn:
-            return ops.apply(y, norm.A, norm.B, per_sample=False, **kw)
-        return ops.apply(y, gn=norm.n.gn(st, _count(y)), **kw)
+                              post=dict(**norm.apply_args(st, Ho * Wo * cw.cout / G), **kw))
 
     def __call__(self, x4):
         """x4 (N,1,H,W,4) normalised image, channels-last padded -> (N,1,H/32,W/32,C) fp32."""
         N, dev = x4.shape[0], x4.device
         st = ops.new_stats(N, G, dev) if self.gn else None
         y = ops.conv_direct(x4, self.stem_w, 2, 3, self.stem_b, stats=st)
-        y = self._napply(self.bn1, y, st, act=ops.ACT_RELU, want_f32=True, want_split=False)
+        y = ops.apply(y, **self.bn1.apply_args(st, _count(y)), act=ops.ACT_RELU, want_f32=True, want_split=False)
         x = ops.maxpool2d_3x3s2(y)
         xs = ops.split_bf16(x, self.planes)
         relu = dict(act=ops.ACT_RELU)
@@ -258,7 +247,7 @@ class ResNet:
                 r, std = self._conv(xs, blk["cd"], s)
                 A2, B2 = blk["nd"].affine(std, _count(r))
                 # residual affine is per-channel in the kernel; with GN and N == 1 the per-sample row is that vector
-                assert last_n.is_bn or N == 1, "GN ResNet path runs one image at a time"
+                assert not last_n.needs_stats or N == 1, "GN ResNet path runs one image at a time"
                 x, xs = self._conv_norm(a, last_c, last_n, last_s, res=r, A2=A2, B2=B2, want_f32=True, want_split=True, **relu)
             else:
                 x, xs = self._conv_norm(a, last_c, last_n, last_s, res=x, want_f32=True, want_split=True, **relu)

@@ -1,7 +1,8 @@
 """Stage-2 refinement path (SURVEY.md §8 row a17 / (f) rank 1): drop-in for `notebooks/infer_s2.py:53-387`
 InferenceWrapper.forward — `LocalEncoderOld` (`networks/volumetric_avatar/local_encoder_old.py:25-117`) followed by
 `Decoder_stage2` / `ImageDecoder_stage2` (`decoder_s2_old.py:18-217, 346-475`), built as in
-`models/stage_2/base/volumetric_avatar_two.py:338-444`, all on the same sm_90a kernels as stage 1.
+`models/stage_2/base/volumetric_avatar_two.py:338-444`, all on the same sm_90a kernels as stage 1.  Every residual block is
+the stage-1 `nets.ResBlock`; its `nets.Norm` is here the folded BatchNorm, so the blocks carry no statistics.
 
 Default stage-2 configuration (argparse defaults of volumetric_avatar_two.py — the shipped stage-2 args.txt is a
 download): norm 'bn' (eval-mode BatchNorm == per-channel affine, folded at load), spectral norm on every conv, no weight
@@ -20,7 +21,7 @@ from typing import Optional
 import torch
 
 from . import nets, ops
-from .checkpoint import _fill, _sn, fold_conv
+from .checkpoint import _fill, _sn
 from .config import parse_args
 
 
@@ -142,58 +143,6 @@ def synthetic_state_dict_s2(cfg: Stage2Config, seed: int = 0):
 # ------------------------------------------------------------------------------------------------------------------
 # networks
 # ------------------------------------------------------------------------------------------------------------------
-class _BN:
-    """eval-mode BatchNorm2d folded to y = x*A + B (per channel)"""
-
-    def __init__(self, sd, p, dev):
-        g, b = sd[p + ".weight"].float(), sd[p + ".bias"].float()
-        m, v = sd[p + ".running_mean"].float(), sd[p + ".running_var"].float()
-        A = g / torch.sqrt(v + 1e-5)
-        self.A = A[None].to(dev).contiguous()
-        self.B = (b - m * A)[None].to(dev).contiguous()
-
-
-class ResBlockBN:
-    """utils.py:661-788 with norm_layer_type 'bn' in eval mode: no statistics are needed, the norm is an affine."""
-
-    def __init__(self, sd, p, dev, planes=2, subpixel_up=False, pool_fold=False):
-        self.planes = planes
-        self.n1 = _BN(sd, p + ".block_feats.0", dev)
-        self.c1 = nets.ConvW(sd, p + ".block_feats.2", dev, planes=planes)
-        self.c1_ps = None  # sub-pixel form of `nearest x2 -> bn -> relu -> 3x3 conv` (see nets.ResBlock)
-        if subpixel_up and planes == 2:
-            w, _ = fold_conv(sd, p + ".block_feats.2")
-            if tuple(w.shape[2:]) == (3, 3) and w.shape[0] % 32 == 0 and w.shape[1] % 64 == 0:
-                self.c1_ps = ops.pack_upconv_weight(w, device=dev)
-        self.n2 = _BN(sd, p + ".block_feats.3", dev)
-        self.c2 = nets.ConvW(sd, p + ".block.0", dev, planes=planes)
-        self.skip = nets.ConvW(sd, p + ".skip.0", dev, planes=planes) if (p + ".skip.0.weight_orig") in sd else None
-        self.c2_pool = None  # `conv -> avgpool (1,2,2)` as one 4x4 stride-2 conv (see nets.ResBlock)
-        if pool_fold:
-            w, _ = fold_conv(sd, p + ".block.0")
-            if tuple(w.shape[2:]) == (3, 3):
-                self.c2_pool = ops.pack_conv_weight(ops.fold_poolconv_weight(w), device=dev, planes=planes)
-
-    def __call__(self, x, up=1, down=None):
-        P = self.planes
-        if up == 2 and self.c1_ps is not None and x.shape[1] == 1 and (x.shape[0] * x.shape[2] * x.shape[3]) % 256 == 0:
-            a = ops.apply(x, self.n1.A, self.n1.B, per_sample=False, act=ops.ACT_RELU, up=1, planes=P)
-            y = ops.conv_igemm(a, self.c1_ps, bias=self.c1.b, upconv=True)
-        else:
-            a = ops.apply(x, self.n1.A, self.n1.B, per_sample=False, act=ops.ACT_RELU, up=up, planes=P)
-            y = ops.conv_igemm(a, self.c1.w, bias=self.c1.b)
-        b = ops.apply(y, self.n2.A, self.n2.B, per_sample=False, act=ops.ACT_RELU, planes=P)
-        s = ops.avgpool(x, down) if down else x
-        if self.skip is not None:
-            s = ops.conv_igemm(ops.split_bf16(s, P), self.skip.w, bias=self.skip.b)
-        if down and self.c2_pool is not None and tuple(down) == (1, 2, 2) and b.shape[2] % 2 == 0 and b.shape[3] % 2 == 0:
-            return ops.conv_igemm(b, self.c2_pool, stride=(1, 2, 2), pad=(0, 1, 1), bias=self.c2.b, residual=s)
-        if down:
-            full = ops.conv_igemm(b, self.c2.w, bias=self.c2.b)
-            return ops.avgpool(full, down, add=s)
-        return ops.conv_igemm(b, self.c2.w, bias=self.c2.b, residual=s, res_shift=1 if up == 2 else 0)
-
-
 class Stage2Model:
     """`model_two.local_encoder` + `model_two.decoder` of notebooks/infer_s2.py:371-372."""
 
@@ -205,23 +154,21 @@ class Stage2Model:
         self.planes = planes
         p = "local_encoder"
         s = cfg.output_size
-        w, b = fold_conv(sd, f"{p}.from_rgb_{s}px")
-        wc = torch.zeros(7, 7, 4, w.shape[0])
-        wc[:, :, :3] = w.permute(2, 3, 1, 0)
-        self.stem_w, self.stem_b = wc.to(dev).contiguous(), b.to(dev).contiguous()
+        self.stem_w, self.stem_b = nets.stem_weight(sd, f"{p}.from_rgb_{s}px", dev)
         self.enc = []
         for i in range(len(cfg.enc_channels) - 1):
-            self.enc.append(ResBlockBN(sd, f"{p}.enc_{i}_block={s}px", dev, planes, pool_fold=True))
+            self.enc.append(nets.ResBlock(sd, f"{p}.enc_{i}_block={s}px", dev, ws_first=False, planes=planes, pool_fold=True))
             s //= 2
-        self.fin_norm = _BN(sd, p + ".finale_layers.0", dev)
+        self.fin_norm = nets.Norm(sd, p + ".finale_layers.0", dev)
         self.fin = nets.ConvW(sd, p + ".finale_layers.2", dev, planes=planes)
         p = "decoder"
         self.inp = nets.ConvW(sd, p + ".res_decoder.0", dev, planes=planes)
-        self.res = [ResBlockBN(sd, f"{p}.res_decoder.{i + 1}", dev, planes) for i in range(cfg.dec_num_blocks)]
-        ps = True
-        self.up = [ResBlockBN(sd, f"{p}.img_decoder.dec_img_blocks.{i}", dev, planes, subpixel_up=ps) for i in range(len(cfg.up_channels) - 1)]
-        self.feat = [ResBlockBN(sd, f"{p}.img_decoder.dec_img_feat_blocks.{i}", dev, planes, subpixel_up=ps and i == 0) for i in range(4)]
-        self.head_norm = _BN(sd, p + ".img_decoder.dec_img_head.0", dev)
+        self.res = [nets.ResBlock(sd, f"{p}.res_decoder.{i + 1}", dev, ws_first=False, planes=planes) for i in range(cfg.dec_num_blocks)]
+        self.up = [nets.ResBlock(sd, f"{p}.img_decoder.dec_img_blocks.{i}", dev, ws_first=False, planes=planes, subpixel_up=True)
+                   for i in range(len(cfg.up_channels) - 1)]
+        self.feat = [nets.ResBlock(sd, f"{p}.img_decoder.dec_img_feat_blocks.{i}", dev, ws_first=False, planes=planes, subpixel_up=i == 0)
+                     for i in range(4)]
+        self.head_norm = nets.Norm(sd, p + ".img_decoder.dec_img_head.0", dev)
         self.head = nets.ConvW(sd, p + ".img_decoder.dec_img_head.2", dev, planes=planes)
 
     @torch.no_grad()
@@ -229,8 +176,8 @@ class Stage2Model:
         """x4 (N,1,S,S,4) channels-last (masked, resized) image -> latent (N,1,64,64,C*depth)"""
         x = ops.conv_direct(x4, self.stem_w, 1, 3, self.stem_b)
         for blk in self.enc:
-            x = blk(x, down=(1, 2, 2))
-        a = ops.apply(x, self.fin_norm.A, self.fin_norm.B, per_sample=False, act=ops.ACT_RELU, planes=self.planes)
+            x, _ = blk(x, down=(1, 2, 2))
+        a = ops.apply(x, **self.fin_norm.apply_args(), act=ops.ACT_RELU, planes=self.planes)
         return ops.conv_igemm(a, self.fin.w, bias=self.fin.b)
 
     @torch.no_grad()
@@ -239,13 +186,13 @@ class Stage2Model:
         P = self.planes
         x = ops.conv_igemm(ops.split_bf16(vol, P), self.inp.w)
         for blk in self.res:
-            x = blk(x)
+            x, _ = blk(x)
         for blk in self.up:
-            x = blk(x, up=2)
-        x = self.feat[0](x, up=2)
+            x, _ = blk(x, up=2)
+        x, _ = self.feat[0](x, up=2)
         for blk in self.feat[1:]:
-            x = blk(x)
-        a = ops.apply(x, self.head_norm.A, self.head_norm.B, per_sample=False, act=ops.ACT_RELU, planes=P)
+            x, _ = blk(x)
+        a = ops.apply(x, **self.head_norm.apply_args(), act=ops.ACT_RELU, planes=P)
         out = ops.conv_igemm(a, self.head.w, bias=self.head.b, act=ops.ACT_TANH, out_nchw=True)
         return out[:, :, 0]
 

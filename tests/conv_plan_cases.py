@@ -69,9 +69,11 @@ CASES = [
     Case("conv<64,2> BN80 rr3 apply", 64, 160, (96, 40), post=True, stats=True),
     Case("conv<64,2> BN80 tap none", 64, 160, (96, 40), k=1, out_nchw=True),
     Case("conv<64,2> BN64 rr3 none", 64, 64, (96, 96), stats=True),
+    Case("conv<64,2> BN64 rr3 apply", 64, 64, (96, 96), post=True, stats=True),
     Case("conv<64,2> BN16 rr3 none", 64, 320, (16, 32), split_k=False, stats=True),            # BN 16 % cpg 10: per-column stats
     Case("conv<64,2> BN64 tap none", 64, 64, (96, 96), k=1, residual=True),
     Case("conv<64,2> BN32 rr3 none", 64, 32, (96, 96), stats=True, G=8),
+    Case("conv<64,2> BN32 rr3 apply", 64, 32, (96, 96), post=True, stats=True),
     Case("conv<64,2> BN32 tap none", 64, 32, (96, 96), k=1, stats=True),
     # bf16 two planes, KC = 32 (Cin % 64 != 0)
     Case("conv<32,2> BN96 rr3 none", 96, 96, (96, 96), residual=True, res_shift=1, stats=True),
