@@ -1,0 +1,435 @@
+"""GPU sweep of the non-convolution kernels: every case of tests/op_cases.py (one per kernel variant, see
+tests/test_op_cases_cpu.py) against a float64 torch reference of the same op, and the GroupNorm edge cases.
+
+Per case: every output starts as NaN inside an allocation whose NaN tail is a guard region; after the call every element of the
+output is written and the guard is untouched.  Outputs match float64 within 2e-5 of their scale (the largest value the kernel
+adds or produces), operand planes within their format's reconstruction bound and bit for bit equal to the host split of the
+kernel's own fp32 output where both are written, and exact ops (max pooling, the same-size repack, factor-1 resampling, the
+splits) match bit for bit.
+
+GroupNorm: every statistics producer on data far from zero mean, normalised by the fused apply and compared with float64
+F.group_norm of the producer's own fp32 output (so that only the statistics' error counts); the finalisation's copies agree."""
+import math
+
+import pytest
+import torch
+import torch.nn.functional as F
+
+import op_cases as OC
+
+pytestmark = pytest.mark.gpu
+GUARD = 4096
+TOL = 2e-5
+# reconstruction bound of each operand-plane format: |planes - y| <= REL * |y| + ABS
+PLANE_BOUND = {"bf16x2": (2.0 ** -16, 0.0), "bf16x3": (2.0 ** -23, 0.0), "fp16x2": (2.0 ** -20, 2.0 ** -28), "fp16x1": (2.0 ** -11, 2.0 ** -28)}
+_WORST = {}   # kernel -> (largest error / max(1, scale), case id)
+
+
+@pytest.fixture(scope="module")
+def ops():
+    from emoportraits_b200 import ops as o
+    return o
+
+
+def _note(kernel, rel, cid):
+    if rel > _WORST.get(kernel, (-1.0, ""))[0]:
+        _WORST[kernel] = (rel, cid)
+
+
+def _alloc(shape, dtype, fill=float("nan"), planes=1):
+    """NaN-guarded output: `planes` tensors of `shape` (stacked as (planes, ...shape) when planes > 1), each followed by its
+    own GUARD elements of NaN; returns (the guard regions (planes, GUARD), the output view)"""
+    n = math.prod(shape)
+    buf = torch.full((planes, n + GUARD), fill, dtype=dtype, device="cuda")
+    buf[:, n:] = float("nan")
+    out = buf[:, :n].view((planes,) + tuple(shape))
+    return buf[:, n:], out if planes > 1 else out[0]
+
+
+def _bits(t):
+    return t.view(torch.int16) if t.element_size() == 2 else t.view(torch.int32) if t.element_size() == 4 else t.view(torch.int64)
+
+
+def host_planes(y, fmt):
+    """the operand planes of fp32 y as the kernels split them"""
+    if fmt.startswith("bf16"):
+        hi = y.bfloat16()
+        r = y - hi.float()
+        lo = r.bfloat16()
+        return torch.stack([hi, lo, (r - lo.float()).bfloat16()][: int(fmt[-1])])
+    ys = (y * OC.F16_SCALE).clamp(-65000.0, 65000.0)
+    hi = ys.half()
+    return torch.stack([hi, (ys - hi.float()).half()][: int(fmt[-1])])
+
+
+def reconstruct(planes, fmt):
+    return planes.double().sum(0) / (OC.F16_SCALE if fmt.startswith("fp16") else 1.0)
+
+
+def _act(y, act):
+    return [lambda v: v, torch.relu, torch.sigmoid, torch.tanh][act](y)
+
+
+def _cl(x):
+    return x.permute(0, 2, 3, 4, 1)
+
+
+def _ncdhw(x):
+    return x.permute(0, 4, 1, 2, 3)
+
+
+def _gn_affine(stats, count, gamma, beta, ada_w=None, ada_b=None, eps=1e-5):
+    """float64 (A, B) [N][C] of a GroupNorm (+ adaptive) from (sum, sum of squares) statistics"""
+    N, G, _ = stats.shape
+    C = gamma.numel()
+    mean = stats[..., 0] / count
+    var = stats[..., 1] / count - mean * mean
+    rstd = (var.clamp_min(0) + eps).rsqrt().repeat_interleave(C // G, 1)
+    mean = mean.repeat_interleave(C // G, 1)
+    gam, bet = gamma.double()[None].expand(N, C), beta.double()[None].expand(N, C)
+    if ada_w is not None:
+        bet, gam = bet * ada_w.double() + ada_b.double(), gam * ada_w.double()
+    A = rstd * gam
+    return A, bet - mean * A
+
+
+def reference(c, t):
+    """{output: float64 reference} and the scale the errors are relative to"""
+    k = c.k
+    if c.op == "apply":
+        x = t["x"].double()
+        N, C = k["N"], k["C"]
+        terms = [x]
+        if "A" in t:
+            A, B = t["A"].double(), t["B"].double()
+        elif "stats" in t:
+            A, B = _gn_affine(t["stats"], t["x"][0].numel() / t["stats"].shape[1], t["gamma"], t["beta"], t.get("ada_w"), t.get("ada_b"))
+        else:
+            A, B = torch.ones(1, C, dtype=torch.float64, device=x.device), torch.zeros(1, C, dtype=torch.float64, device=x.device)
+        bs = (A.shape[0], 1, 1, 1, C)
+        y = x * A.view(bs) + B.view(bs)
+        terms += [y, x * A.view(bs)]
+        if "res" in t:
+            r = t["res"].double()
+            if "A2" in t:
+                r = r * t["A2"].double() + t["B2"].double()
+            terms.append(r)
+            y = y + r
+        y = _act(y, k["act"])
+        if k["up"] == 2:
+            y = y.repeat_interleave(2, 2).repeat_interleave(2, 3)
+        return {"y": y}, max(v.abs().max().item() for v in terms)
+    if c.op == "gn_stats":
+        N, C, G = k["N"], k["C"], k["G"]
+        r = t["x"].double().reshape(N, -1, G, C // G)
+        return {"stats": torch.stack([r.sum((1, 3)), (r * r).sum((1, 3))], -1), "abs": r.abs().sum((1, 3))}, 1.0
+    if c.op == "gn_finalize":
+        A, B = _gn_affine(t["stats"], t["count"], t["gamma"], t["beta"], t.get("ada_w"), t.get("ada_b"))
+        return {"A": A, "B": B}, max(A.abs().max().item(), B.abs().max().item())
+    if c.op == "gn_head":
+        x = t["x"].double().flatten(1, 3)                                        # (N, S, C)
+        A, B = _gn_affine(t["stats"], x[0].numel() / 32, t["gamma"], t["beta"])
+        h = torch.relu(x * A[:, None] + B[:, None])
+        pre = torch.einsum("nsc,oc->nos", h, t["w"].double()) + t["bias"].double()[None, :, None]
+        scale = torch.einsum("nsc,oc->nos", h, t["w"].double().abs()).max().item() + t["bias"].abs().max().item()
+        return {"out": _act(pre, k["act"])}, scale
+    if c.op == "grid_sample3d":
+        x = t["x"].double()
+        x = x if k["layout"] == "ncdhw" else _ncdhw(x)
+        if "theta" in t:
+            Do, Ho, Wo = k["outs"]
+            zs, ys, xs = (torch.linspace(-1, 1, n, dtype=torch.float64, device=x.device) for n in (Do, Ho, Wo))
+            w, v, u = torch.meshgrid(zs, ys, xs, indexing="ij")
+            lat = torch.stack([u, v, w, torch.ones_like(u)], -1)
+            grid = torch.einsum("dhwj,nij->ndhwi", lat, t["theta"].double())
+        else:
+            grid = t["grid"].double()
+        y = F.grid_sample(x, grid, mode="bilinear", padding_mode="zeros", align_corners=False)
+        y = {"ncdhw": y, "cl": _cl(y), "hwdc": y.permute(0, 3, 4, 2, 1)}[k["out_layout"]]
+        return {"y": y}, x.abs().max().item()
+    if c.op in ("upsample_trilinear", "avgpool"):
+        x = _ncdhw(t["x"].double())
+        f = k["f"]
+        y = F.interpolate(x, scale_factor=f, mode="trilinear", align_corners=False) if c.op == "upsample_trilinear" \
+            else F.avg_pool3d(x, f, f)
+        y = _cl(y)
+        if "add" in t:
+            y = y + t["add"].double()
+        return {"out": y}, max(x.abs().max().item(), y.abs().max().item())
+    if c.op == "linear":
+        M, Nn, K = k["M"], k["N"], k["K"]
+        X = t["x"].double().as_strided((M, K), k["xs"])
+        y = X @ t["w"].double().T
+        scale = (X.abs() @ t["w"].double().abs().T).max().item()
+        if "bias" in t:
+            y = y + t["bias"].double()
+        out = torch.full(OC.out_specs(c)["out"][0], float("nan"), dtype=torch.float64, device=X.device)
+        ov = out.as_strided((M, Nn), k["os"])
+        if "add" in t:
+            y = y + t["add"].double().as_strided((M, Nn), k["os"])
+        ov.copy_(_act(y * k["scale"], k["act"]))
+        return {"out": out}, max(scale, y.abs().max().item()) * max(1.0, k["scale"])
+    if c.op == "conv_direct":
+        x = t["x"].double()[:, 0].permute(0, 3, 1, 2)
+        w = t["w"].double().permute(3, 2, 0, 1)
+        y = F.conv2d(x, w, t["bias"].double(), stride=k["stride"], padding=OC.kk_pad(c))
+        scale = F.conv2d(x.abs(), w.abs(), t["bias"].double().abs(), stride=k["stride"], padding=OC.kk_pad(c)).max().item()
+        return {"out": y.permute(0, 2, 3, 1)[:, None]}, scale
+    if c.op == "maxpool2d_3x3s2":
+        x = t["x"][:, 0].permute(0, 3, 1, 2)
+        return {"out": F.max_pool2d(x, 3, 2, 1).permute(0, 2, 3, 1)[:, None]}, 1.0
+    if c.op == "global_avgpool":
+        return {"out": t["x"].double().mean(1)}, t["x"].abs().max().item()
+    if c.op in ("resize_bilinear", "grid_sample2d_affine"):
+        x = t["x"].double()
+        if c.op == "resize_bilinear":
+            y = F.interpolate(x, size=k["outs"], mode="bilinear", align_corners=False)
+        else:
+            Ho, Wo = k["outs"]
+            ys, xs = (torch.linspace(-1, 1, n, dtype=torch.float64, device=x.device) for n in (Ho, Wo))
+            v, u = torch.meshgrid(ys, xs, indexing="ij")
+            grid = torch.einsum("hwj,nij->nhwi", torch.stack([u, v, torch.ones_like(u)], -1), t["theta"].double())
+            y = F.grid_sample(x, grid, mode="bilinear", padding_mode="zeros", align_corners=False)
+        ref = {"nchw": y}
+        if "mean" in t:
+            y = (y - t["mean"].double()[None, :, None, None]) / t["std"].double()[None, :, None, None]
+        out = torch.zeros((k["N"], 1) + k["outs"] + (k["C_pad"],), dtype=torch.float64, device=x.device)
+        out[:, 0, ..., : k["C"]] = y.permute(0, 2, 3, 1)
+        ref["out"] = out
+        return ref, max(1.0, y.abs().max().item())
+    if c.op in ("split_bf16", "split_f16"):
+        return {"y": t["x"].double()}, 1.0
+    raise KeyError(c.op)
+
+
+@pytest.mark.parametrize("c", OC.CASES, ids=[c.id for c in OC.CASES])
+def test_op_case_against_float64(ops, c):
+    from emoportraits_b200 import lib as L
+
+    t = OC.inputs(c, "cuda")
+    guards, o = {}, {}
+    for name, (shape, dt) in OC.out_specs(c).items():
+        np_ = shape[0] if name == "planes" else 1          # operand planes: one guard region after each plane
+        guards[name], o[name] = _alloc(shape[1:] if name == "planes" else shape, dt,
+                                       0.0 if name == "stats" else float("nan"), np_)   # statistics accumulate (+=)
+        if name == "planes" and np_ == 1:
+            o[name] = o[name][None]
+    fn, args = OC.launch(c, ops, t, o)
+    L.call(fn, *args)
+    torch.cuda.synchronize()
+    for name, guard in guards.items():
+        assert torch.isnan(guard.float()).all(), f"{name}: write past the end of the output (or of one of its planes)"
+    ref, scale = reference(c, t)
+    bound = TOL * max(1.0, scale)
+    k = c.k
+    msg = f"\n[{c.id}] {c.want}:"
+    kernel = c.want.split(" ")[0] if not c.op.startswith("split") else c.op
+    exact = (c.op == "maxpool2d_3x3s2" or c.op.startswith("split")
+             or (c.op in ("upsample_trilinear", "avgpool") and k["f"] == (1, 1, 1) and not k["add"])
+             or (c.op == "resize_bilinear" and k["ins"] == k["outs"] and not k["norm"]))
+
+    if c.op in ("gn_stats", "upsample_trilinear", "avgpool", "conv_direct") and "stats" in o:
+        st = o["stats"]
+        if c.op == "gn_stats":
+            want, mag = ref["stats"], ref["abs"]
+        else:   # the producer's statistics of its own output
+            y = o["out"].double()
+            r = y.reshape(y.shape[0], -1, st.shape[1], y.shape[-1] // st.shape[1])
+            want, mag = torch.stack([r.sum((1, 3)), (r * r).sum((1, 3))], -1), r.abs().sum((1, 3))
+        es = ((st[..., 0] - want[..., 0]).abs() / mag).max().item()
+        eq = ((st[..., 1] - want[..., 1]).abs() / want[..., 1]).max().item()
+        msg += f" stats: sum {es:.1e} (of sum |x|), sum of squares {eq:.1e} (rel)"
+        _note(c.op + " stats", max(es, eq), c.id)
+        assert es < 2e-6 and eq < 2e-6, (es, eq)
+    if c.op == "gn_stats":
+        print(msg)
+        return
+    for name in ("out", "A", "B", "nchw"):
+        if name in o and name in ref:
+            got = o[name]
+            assert not torch.isnan(got).any() or c.op == "linear", f"{name}: {int(torch.isnan(got).sum())} elements never written"
+            want = ref[name]
+            if c.op == "linear":   # only the strided (m, n) positions are written
+                assert torch.equal(torch.isnan(got), torch.isnan(want)), "written positions differ from the (m, n) lattice"
+                got, want = got[~torch.isnan(want)], want[~torch.isnan(want)]
+            if exact:
+                assert torch.equal(got.double(), want), f"{name}: not bit-exact"
+            e = (got.double() - want).abs().max().item()
+            msg += f" {name} max-abs {e:.2e} (scale {scale:.2f})"
+            _note(kernel, e / max(1.0, scale), c.id)
+            assert e < bound, (name, e, bound)
+            if c.op in ("resize_bilinear", "grid_sample2d_affine") and name == "out":
+                assert (got[..., k["C"]:] == 0).all(), "padding channels not zero"
+    fmt = next((p for p in (k.get("out") or ()) if p != "fp32"), None) if c.op == "apply" else \
+        (k["planes"] if k["planes"] != "none" else None) if c.op == "grid_sample3d" else \
+        ({"split_bf16": "bf16x", "split_f16": "fp16x"}[c.op] + str(k["planes"])) if c.op.startswith("split") else None
+    if "y" in ref and "out" in o and c.op in ("apply", "grid_sample3d"):
+        got = o["out"]
+        assert not torch.isnan(got).any(), f"{int(torch.isnan(got).sum())} output elements never written"
+        e = (got.double() - ref["y"]).abs().max().item()
+        msg += f" fp32 max-abs {e:.2e} (scale {scale:.2f})"
+        _note(kernel, e / max(1.0, scale), c.id)
+        assert e < bound, (e, bound)
+    if fmt is not None:
+        planes = o["planes"]
+        assert not torch.isnan(planes.float()).any(), f"{int(torch.isnan(planes.float()).sum())} plane elements never written"
+        rel, ab = PLANE_BOUND[fmt]
+        y = ref["y"]
+        e = ((reconstruct(planes, fmt) - y).abs() - rel * y.abs() - ab).max().item()
+        msg += f" {fmt} planes: excess over the format bound {e:.2e}"
+        assert e <= (bound if not c.op.startswith("split") else 0.0), (fmt, e, bound)
+        src = o.get("out") if "out" in o else (t["x"] if c.op.startswith("split") else None)
+        if src is not None:
+            assert torch.equal(_bits(planes.contiguous()), _bits(host_planes(src, fmt))), "planes differ from the split of the fp32 output"
+            msg += " (bit-equal to the split of the fp32 values)"
+    print(msg)
+
+
+def test_report_largest_error_per_kernel():
+    """(runs after the sweep) the largest error / max(1, scale) seen per kernel"""
+    if not _WORST:
+        pytest.skip("no sweep case ran")
+    for k, (rel, cid) in sorted(_WORST.items()):
+        print(f"\n[largest relative error] {k:36s} {rel:.2e}  ({cid})", end="")
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# GroupNorm on data far from zero mean
+# ------------------------------------------------------------------------------------------------------------------
+RATIOS = (0.0, 3.0, 10.0, 30.0, 100.0)
+_GN_TABLE = {}
+
+
+def _offset_groups(y, G):
+    """group 0 of every sample constant 3.0, group 1 all zero (a dead ReLU): the degenerate groups of real activations"""
+    cpg = y.shape[-1] // G
+    y[..., :cpg] = 3.0
+    y[..., cpg:2 * cpg] = 0.0
+    return y
+
+
+def _producer(ops, name, r):
+    """(fp32 channels-last output of the producer, its statistics, G, normalised output of a fused post-op or None) for data
+    offset by r (added to the input, or to the convolution's bias)"""
+    g = torch.Generator().manual_seed(7)
+    G = 32
+    if name == "gn_stats":
+        x = _offset_groups(torch.randn(2, 1, 40, 40, 96, generator=g) + r, G).cuda()
+        return x, ops.gn_stats(x, G, stats=torch.zeros(2, G, 2, dtype=torch.float64, device="cuda")), G, None
+    if name in ("upsample", "avgpool"):
+        x = _offset_groups(torch.randn(2, 6, 12, 10, 64, generator=g) + r, G).cuda()
+        st = torch.zeros(2, G, 2, dtype=torch.float64, device="cuda")
+        y = ops.upsample_trilinear(x, (2, 2, 2), stats=st, G=G) if name == "upsample" else ops.avgpool(x, (2, 2, 2), stats=st, G=G)
+        return y, st, G, None
+    if name == "conv_direct":
+        x = torch.zeros(2, 1, 32, 32, 4)
+        x[..., :3] = torch.rand(2, 1, 32, 32, 3, generator=g) * 2 - 1
+        w = torch.zeros(7, 7, 4, 64)
+        w[:, :, :3] = torch.randn(7, 7, 3, 64, generator=g) / math.sqrt(49)
+        w[..., :4] = 0.0                                            # groups 0 (constant 3.0) and 1 (zero) of G = 32
+        b = torch.full((64,), r)
+        b[:2], b[2:4] = 3.0, 0.0
+        st = torch.zeros(2, G, 2, dtype=torch.float64, device="cuda")
+        y = ops.conv_direct(x.cuda(), w.cuda(), 1, 3, b.cuda(), stats=st, G=G)
+        return y, st, G, None
+    # the convolution's statistics: tile epilogue (per-group and per-column), split-K finalize, fused split-K post kernel
+    Cin, Cout, sp, planes, split_k = {"conv per-group": (64, 64, (48, 48), 2, False), "conv per-column": (64, 320, (16, 32), 2, False),
+                                      "split-K finalize": (256, 256, (8, 8), 2, True),
+                                      "split-K post": (256, 256, (8, 8), "h2", True)}[name]
+    x = torch.randn(1, 1, *sp, Cin, generator=g)
+    w = torch.randn(Cout, Cin, 3, 3, generator=g) / math.sqrt(9 * Cin)
+    cpg = Cout // G
+    w[: 2 * cpg] = 0.0
+    b = torch.full((Cout,), r)
+    b[:cpg], b[cpg:2 * cpg] = 3.0, 0.0
+    a, pw = ops.split_bf16(x.cuda(), planes), ops.pack_conv_weight(w, planes=planes)
+    st = torch.zeros(1, G, 2, dtype=torch.float64, device="cuda")
+    y = ops.conv_igemm(a, pw, bias=b.cuda(), stats=None if name == "split-K post" else st, split_k=split_k)
+    if name != "split-K post":
+        return y, st, G, None
+    # the fused kernel writes the post-op's output only; `y` (the finalize path, the same part order) is its input
+    ones, zeros = torch.ones(Cout, device="cuda"), torch.zeros(Cout, device="cuda")
+    post = dict(act=0, planes=planes, want_f32=True, want_split=False,
+                gn=dict(stats=st, count=y[0].numel() / G, gamma=ones, beta=zeros))
+    info = ops.conv_plan(a, pw, bias=b.cuda(), stats=st, post=post)
+    assert info.finish == 2, info.finish                             # EMO_CONV_FINISH_POST
+    z = ops.conv_igemm(a, pw, bias=b.cuda(), stats=st, post=post)
+    return y, st, G, z
+
+
+PRODUCERS = ("gn_stats", "conv per-group", "conv per-column", "split-K finalize", "split-K post", "conv_direct", "upsample", "avgpool")
+
+
+def _group_moments(y, G):
+    """per-(sample, group) mean and standard deviation of a channels-last tensor, float64"""
+    t = y.double().reshape(y.shape[0], -1, G, y.shape[-1] // G).transpose(1, 2).flatten(2)
+    return t.mean(-1), t.std(-1, unbiased=False)
+
+
+@pytest.mark.parametrize("r", RATIOS)
+@pytest.mark.parametrize("producer", PRODUCERS)
+def test_groupnorm_offset_data(ops, producer, r):
+    """normalised output of offset data (largest per-group mean / std = r, plus one constant and one all-zero group) through
+    each statistics producer, against float64 F.group_norm of the producer's own fp32 output: the 2e-5 bar is asserted up
+    to op_cases.GN_ASSERTED_RATIO, larger ratios are reported only.  The offset (added to every group but the two degenerate
+    ones) is the smallest r * std - mean over the groups of the producer's un-offset output, so that the largest mean / std
+    of the offset output is r."""
+    off = 0.0
+    if r > 0:
+        y0, _, G, _ = _producer(ops, producer, 0.0)
+        m0, s0 = _group_moments(y0, G)
+        off = (r * s0 - m0)[:, 2:].min().item()
+    y, st, G, z = _producer(ops, producer, off)
+    C = y.shape[-1]
+    if z is None:
+        ones, zeros = torch.ones(C, device="cuda"), torch.zeros(C, device="cuda")
+        z = ops.apply(y, gn=dict(stats=st, count=y[0].numel() / G, gamma=ones, beta=zeros), want_f32=True, want_split=False)
+    torch.cuda.synchronize()
+    ref = _cl(F.group_norm(_ncdhw(y.double()), G, eps=1e-5))
+    mean, std = _group_moments(y, G)
+    ratio = (mean.abs() / std)[std > 0].max().item()
+    err = (z.double() - ref).abs().max().item()
+    degenerate = (z.double() - ref).abs()[..., : 2 * (C // G)].max().item()
+    _GN_TABLE[(producer, r)] = (err, ratio)
+    print(f"\n[GroupNorm offset data] {producer:17s} mean/std {ratio:6.1f}: normalised-output error {err:.2e} "
+          f"(constant and zero groups {degenerate:.1e})")
+    assert degenerate < TOL, degenerate
+    assert abs(ratio - r) < 0.01 * r + 0.5, ratio                       # the table is keyed on the achieved ratio
+    if r <= OC.GN_ASSERTED_RATIO:
+        assert err < TOL, (err, ratio)
+
+
+def test_report_groupnorm_table():
+    """(runs after the offset sweep) normalised-output error per producer x mean/std"""
+    if not _GN_TABLE:
+        pytest.skip("no offset case ran")
+    print("\n[GroupNorm normalised-output error] producer" + "".join(f"  r={r:<7g}" for r in RATIOS), end="")
+    for p in PRODUCERS:
+        print(f"\n  {p:17s}" + "".join(f"  {_GN_TABLE[(p, r)][0]:.1e}" if (p, r) in _GN_TABLE else "  -      " for r in RATIOS), end="")
+
+
+@pytest.mark.parametrize("ada", [False, True])
+def test_groupnorm_finalisation_copies_agree(ops, ada):
+    """apply(gn=stats) derives the affine in the kernel; apply(A, B = gn_finalize(stats)) reads it: bit for bit the same.
+    gn_head (the fused image head) equals apply -> ReLU -> 1x1 in float64 within 2e-5."""
+    g = torch.Generator().manual_seed(21 + ada)
+    N, C = 2, 96
+    x = (torch.randn(N, 2, 12, 20, C, generator=g) * 1.7 + 2.5).cuda()
+    gamma, beta = (torch.rand(C, generator=g) + 0.5).cuda(), torch.randn(C, generator=g).cuda()
+    aw, ab = ((torch.rand(N, C, generator=g) + 0.5).cuda(), torch.randn(N, C, generator=g).cuda()) if ada else (None, None)
+    st = ops.gn_stats(x, 32, stats=torch.zeros(N, 32, 2, dtype=torch.float64, device="cuda"))
+    count = x[0].numel() / 32
+    fused = ops.apply(x, gn=dict(stats=st, count=count, gamma=gamma, beta=beta, ada_w=aw, ada_b=ab), act=1, want_f32=True,
+                      want_split=False)
+    A, B = ops.gn_finalize(st, count, gamma, beta, ada_w=aw, ada_b=ab)
+    split = ops.apply(x, A, B, act=1, want_f32=True, want_split=False)
+    torch.cuda.synchronize()
+    assert torch.equal(fused, split)
+    if ada:
+        return
+    w, b = (torch.randn(3, C, generator=g) / C ** 0.5).cuda(), torch.randn(3, generator=g).cuda()
+    head = ops.gn_head(x, dict(stats=st, count=count, gamma=gamma, beta=beta), w, b)
+    want = torch.einsum("ndhwc,oc->nodhw", fused.double(), w.double()) + b.double()[None, :, None, None, None]
+    e = (head.double() - want).abs().max().item()
+    print(f"\n[GroupNorm copies] gn_head vs apply -> 1x1: {e:.2e}")
+    assert e < TOL, e
