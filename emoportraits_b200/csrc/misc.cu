@@ -111,6 +111,27 @@ __global__ void __launch_bounds__(256) conv_direct_kernel(const emo_conv_direct_
 }
 
 // ------------------------------------------------------------------------------------------------
+// RGB stem operand for the tensor cores: thread = one pixel.  Its 7 horizontal taps (float4 each, neighbouring threads read
+// overlapping taps through L1) become 28 fp16 channels of (value * scale), then 4 zero channels: 64 bytes, 4 x 16-byte stores.
+// ------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) stem_pack_kernel(const float4* __restrict__ x, int H, int W, long long pixels, float s,
+                                                       uint4* __restrict__ out) {
+  for (long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x; p < pixels; p += (long long)gridDim.x * blockDim.x) {
+    const int w = (int)(p % W);
+    uint2 v[8];
+#pragma unroll
+    for (int kx = 0; kx < 7; ++kx) {
+      const int ix = w + kx - 3;
+      v[kx] = (ix >= 0 && ix < W) ? plane4_h(__ldg(x + p + (kx - 3)), s) : make_uint2(0u, 0u);
+    }
+    v[7] = make_uint2(0u, 0u);
+    uint4* o = out + p * 4;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) o[j] = make_uint4(v[2 * j].x, v[2 * j].y, v[2 * j + 1].x, v[2 * j + 1].y);
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
 // trilinear upsample (align_corners=False), factors in {1,2} per axis, channels-last, optional add + GN stats
 //   src = max((dst + 0.5)/f - 0.5, 0); i0 = floor(src); i1 = min(i0+1, n-1); l = src - i0
 // ------------------------------------------------------------------------------------------------
@@ -358,7 +379,7 @@ extern "C" int emo_composite(const float* img, const float* mask, const float* b
 }
 
 extern "C" const char* emo_last_error(void) { return emo::g_err; }
-extern "C" int emo_version(void) { return 106; }  // 101: emo_pose_desc (+theta_in, mix_old, smoothing) and emo_conv_desc (+upconv) grew trailing fields
+extern "C" int emo_version(void) { return 107; }  // 101: emo_pose_desc (+theta_in, mix_old, smoothing) and emo_conv_desc (+upconv) grew trailing fields
 
 extern "C" int emo_device_info(int* sm_count, int* cc) {
   int dev = 0;
@@ -391,6 +412,20 @@ extern "C" int emo_conv_direct(const emo_conv_direct_desc* d, void* stream_) {
   const long long total = per_n * d->N;
   launch_kernel(conv_direct_kernel, (unsigned)cdivll(total, 256), 256, d->stats ? 2 * d->G * sizeof(double) : 0, stream, *d);
   return check_launch("emo_conv_direct");
+}
+
+extern "C" int emo_stem_pack(const float* x, int N, int H, int W, int C, float scale, void* out, void* stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  EMO_REQUIRE(x && out, "emo_stem_pack: null pointer");
+  EMO_REQUIRE(((uintptr_t)x % 16) == 0 && ((uintptr_t)out % 16) == 0, "emo_stem_pack: x and out must be 16-byte aligned");
+  EMO_REQUIRE(C == 4, "emo_stem_pack: C must be 4 (C=%d)", C);
+  EMO_REQUIRE(N > 0 && H > 0 && W > 0, "emo_stem_pack: bad shape (N=%d H=%d W=%d)", N, H, W);
+  EMO_REQUIRE(scale > 0.f, "emo_stem_pack: scale must be positive");
+  const long long pixels = (long long)N * H * W;
+  long long blocks = cdivll(pixels, 256);
+  if (blocks > 132ll * 16) blocks = 132ll * 16;
+  launch_kernel(stem_pack_kernel, (unsigned)blocks, 256, 0, stream, (const float4*)x, H, W, pixels, scale, (uint4*)out);
+  return check_launch("emo_stem_pack");
 }
 
 static int resample_check(const emo_resample_desc* d, const char* who) {

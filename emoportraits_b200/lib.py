@@ -127,6 +127,7 @@ SYMBOLS = {
     "emo_conv_igemm": (c_int, [C.POINTER(ConvDesc), c_void_p]),
     "emo_conv_plan": (c_int, [C.POINTER(ConvDesc), c_int, C.POINTER(ConvPlanInfo)]),
     "emo_conv_direct": (c_int, [C.POINTER(ConvDirectDesc), c_void_p]),
+    "emo_stem_pack": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p]),
     "emo_linear": (c_int, [C.POINTER(LinearDesc), c_void_p]),
     "emo_upsample_trilinear": (c_int, [C.POINTER(ResampleDesc), c_void_p]),
     "emo_avgpool": (c_int, [C.POINTER(ResampleDesc), c_void_p]),

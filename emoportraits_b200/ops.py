@@ -42,8 +42,8 @@ H2 = "h2"
 F16_ACT_SCALE = 16.0    # activations: post-GroupNorm / ReLU values are O(1)
 F16_W_SCALE = 256.0     # spectral-norm / weight-standardised weights are O(0.01 .. 1)
 # fp16 one-plane operand mode ("h1"): ONE fp16 plane of (value * the same power of two as "h2"), one MMA per product instead of
-# three, ~2^-11 relative per operand.  Decoder only (DESIGN.md section 2): the embedding / warp networks feed the sampler, which
-# amplifies their errors ~100x (tools/decoder_precision_emulation.py gives the decoder's bounds).
+# three, ~2^-11 relative per operand.  Stage 1's decoder and stage 2 only, in their fast modes (DESIGN.md section 2): the embedding
+# / warp networks feed the sampler, which amplifies their errors ~100x (tools/decoder_precision_emulation.py gives the bounds).
 H1 = "h1"
 
 
@@ -554,6 +554,30 @@ def conv_direct(x: torch.Tensor, w: torch.Tensor, stride: int, pad: int, bias=No
                          G if stats is not None else 0)
     L.call("emo_conv_direct", C.byref(d), _stream())
     return out
+
+
+STEM_CIN = 32   # channels of stem_pack()'s plane: 7 horizontal taps x 4 padded RGB channels, then 4 zero channels
+
+
+def stem_pack(x4: torch.Tensor) -> Split:
+    """x4 (N,1,H,W,4) fp32 channels-last (the padded RGB of resize_bilinear) -> one fp16 plane (N,1,H,W,32) of the 7x7 stem's
+    horizontal taps: channel kx*4 + c = fp16(16 x[n, h, w + kx - 3, c]), zero outside the image and in channels 28..31.  The
+    stem then runs on the tensor cores as conv_igemm(stem_pack(x4), pack_stem_weight(w), pad=(0, 3, 0)): a 7x1 convolution."""
+    _chk(x4)
+    N, D, H, W, Cc = x4.shape
+    sp = Split.empty((N, D, H, W, STEM_CIN), x4.device, H1)
+    L.call("emo_stem_pack", _p(x4), N * D, H, W, Cc, C.c_float(sp.scale), _p(sp.hi), _stream())
+    return sp
+
+
+def pack_stem_weight(w_direct: torch.Tensor, device=None) -> PackedConvWeight:
+    """conv_direct weight of a 7x7 stem (7, 7, 4, Cout) [ky][kx][c][o] -> the one-plane weight of the 7x1 convolution over
+    stem_pack()'s channels: [ky][Cout_pad][kx*4 + c] = fp16(256 w[ky][kx][c][o]), zero in channels 28..31."""
+    kh, kw, cp, co = w_direct.shape
+    assert (kh, kw, cp) == (7, 7, 4), w_direct.shape
+    w = torch.zeros(co, STEM_CIN, kh, 1)
+    w[:, :kw * cp, :, 0] = w_direct.detach().float().cpu().permute(3, 1, 2, 0).reshape(co, kw * cp, kh)
+    return pack_conv_weight(w, device=device, planes=H1)
 
 
 def linear(x: torch.Tensor, w: torch.Tensor, bias=None, add=None, scale: float = 1.0, act: int = ACT_NONE,

@@ -143,18 +143,31 @@ def synthetic_state_dict_s2(cfg: Stage2Config, seed: int = 0):
 # ------------------------------------------------------------------------------------------------------------------
 # networks
 # ------------------------------------------------------------------------------------------------------------------
-class Stage2Model:
-    """`model_two.local_encoder` + `model_two.decoder` of notebooks/infer_s2.py:371-372."""
+def _check_precision(precision):
+    if precision not in ("exact", "fast"):
+        raise ValueError(f"precision={precision!r}: 'exact' or 'fast'")
 
-    def __init__(self, cfg: Stage2Config, state_dict, device="cuda", planes: int = 2):
+
+class Stage2Model:
+    """`model_two.local_encoder` + `model_two.decoder` of notebooks/infer_s2.py:371-372.
+
+    precision="exact" runs every implicit-GEMM convolution on two bf16 operand planes and the 7x7 RGB stem as an fp32 SIMT
+    convolution.  precision="fast" runs every convolution on one fp16 plane (ops.H1: one MMA per product), the stem included:
+    ops.stem_pack lays its 7 horizontal taps out as channels, so that it becomes a 7x1 implicit GEMM over 32 channels.  The
+    error budget is DESIGN.md section 2 (tools/decoder_precision_emulation.py --stage2)."""
+
+    def __init__(self, cfg: Stage2Config, state_dict, device="cuda", precision: str = "exact"):
+        _check_precision(precision)
         self.cfg = cfg
         dev = torch.device(device)
         self.device = dev
         sd = state_dict
-        self.planes = planes
+        self.precision = precision
+        self.planes = planes = ops.H1 if precision == "fast" else 2
         p = "local_encoder"
         s = cfg.output_size
         self.stem_w, self.stem_b = nets.stem_weight(sd, f"{p}.from_rgb_{s}px", dev)
+        self.stem_h1 = ops.pack_stem_weight(self.stem_w.cpu(), device=dev) if planes == ops.H1 else None
         self.enc = []
         for i in range(len(cfg.enc_channels) - 1):
             self.enc.append(nets.ResBlock(sd, f"{p}.enc_{i}_block={s}px", dev, ws_first=False, planes=planes, pool_fold=True))
@@ -174,7 +187,10 @@ class Stage2Model:
     @torch.no_grad()
     def local_encoder(self, x4):
         """x4 (N,1,S,S,4) channels-last (masked, resized) image -> latent (N,1,64,64,C*depth)"""
-        x = ops.conv_direct(x4, self.stem_w, 1, 3, self.stem_b)
+        if self.stem_h1 is not None:
+            x = ops.conv_igemm(ops.stem_pack(x4), self.stem_h1, pad=(0, 3, 0), bias=self.stem_b)
+        else:
+            x = ops.conv_direct(x4, self.stem_w, 1, 3, self.stem_b)
         for blk in self.enc:
             x, _ = blk(x, down=(1, 2, 2))
         a = ops.apply(x, **self.fin_norm.apply_args(), act=ops.ACT_RELU, planes=self.planes)
@@ -224,8 +240,11 @@ class InferenceWrapper(torch.nn.Module):
     def __init__(self, experiment_name, which_epoch='latest', model_file_name='', use_gpu=True, num_gpus=1,
                  fixed_bounding_box=False, project_dir='./', torch_home='', debug=False, print_model=False,
                  args_overwrite={}, pose_momentum=0.5, experiment_name_s1=None, model_file_name_s1=None, cloth=False,
-                 state_dict=None):
+                 state_dict=None, precision="exact"):
+        """precision: "exact" (default: the parity path) or "fast" (every convolution on one fp16 plane, INTEGRATION.md
+        "Fast mode"); video.drive_image_with_video runs stage 2 with this setting."""
         super().__init__()
+        _check_precision(precision)
         if not use_gpu or not torch.cuda.is_available():
             raise RuntimeError("emoportraits_b200 stage-2 InferenceWrapper needs a CUDA device; there is no CPU path")
         self.cloth = cloth
@@ -239,7 +258,8 @@ class InferenceWrapper(torch.nn.Module):
         self.model_checkpoint_s2 = pathlib.Path(project_dir) / 'logs_s2' / experiment_name / 'checkpoints' / model_file_name
         if state_dict is None:
             state_dict = torch.load(self.model_checkpoint_s2, map_location='cpu')
-        self.model_two = Stage2Model(self.cfg, state_dict, self.device)
+        self.precision = precision
+        self.model_two = Stage2Model(self.cfg, state_dict, self.device, precision=precision)
 
     @torch.no_grad()
     def forward(self, img, cloth=False, mask=None, face_mask=None):

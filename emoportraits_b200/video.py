@@ -54,7 +54,9 @@ def drive_image_with_video(inferer, source, frames: Sequence, inferer_s2=None, b
     driving frames (PIL).  Returns (list of output PIL images, list of cropped PIL images or None, frames).
     bg (3,H,W) tensor + mask_fn: composite every animated frame over the background (cell 41) before stage 2.
     crop_box = (left, upper, right, lower) on the output: the fixed crop of cell 46 (first-frame face box, computed by the
-    caller's face detector)."""
+    caller's face detector).
+    Each wrapper runs with the `precision=` it was built with: a stage-2 wrapper built with precision="fast" refines every
+    chunk in fast mode, exactly as calling that wrapper on the same chunk would."""
     from PIL import Image
 
     kw = dict(crop=False, smooth_pose=False, target_theta=True, mix=True, mix_old=False, modnet_mask=False)

@@ -35,7 +35,7 @@ extern "C" {
 enum { EMO_ACT_NONE = 0, EMO_ACT_RELU = 1, EMO_ACT_SIGMOID = 2, EMO_ACT_TANH = 3 };
 
 const char* emo_last_error(void);
-int emo_version(void); /* 106: one-plane fp16 operands (emo_conv_desc, emo_apply_desc, emo_grid_sample3d_desc.plane_fp16,
+int emo_version(void); /* 107: + emo_stem_pack; 106: one-plane fp16 operands (emo_conv_desc, emo_apply_desc, emo_grid_sample3d_desc.plane_fp16,
                           emo_split_f16 with lo == NULL) and the EMO_CONV_KERNEL_H1_* kernels; 105: + emo_conv_plan; 104: + emo_composite; 103: emo_conv_desc.post; 102: + emo_u8_to_image, emo_image_to_u8, emo_resize_bicubic; 101: emo_pose_desc and emo_conv_desc gained trailing fields */
 /* sm count, and cc major*10+minor of the current device */
 int emo_device_info(int* sm_count, int* cc);
@@ -299,6 +299,13 @@ typedef struct {
   int G;
 } emo_conv_direct_desc;
 int emo_conv_direct(const emo_conv_direct_desc* d, void* stream);
+
+/* The 7x7 RGB stem as a tensor-core operand (stage-2 fast mode): the 7 horizontal taps of each pixel become 28 channels of one
+ * fp16 plane, so that the stem runs on emo_conv_igemm as a 7x1 convolution over Cin = 32 (pad (3, 0)).
+ * x: fp32 channels-last [N][H][W][C], C == 4 (the padded RGB of emo_resize_bilinear), 16-byte aligned.
+ * out: fp16 [N][H][W][32], 16-byte aligned:  out[n][h][w][kx*4 + c] = fp16(scale * x[n][h][w + kx - 3][c]) for kx = 0..6,
+ *      exactly 0 for columns outside the image and for channels 28..31. */
+int emo_stem_pack(const float* x, int N, int H, int W, int C, float scale, void* out, void* stream);
 
 /* y[m][n] = act((sum_k x[m][k] * w[n][k] + bias[n] + add[m][n]) * scale), fp32 SIMT.
  * Replaces: va.py:820-823 (pose_unsqueeze_nw), :855 (warp_embed_head_orig_nw on a 4x4 map),

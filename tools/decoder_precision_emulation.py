@@ -1,6 +1,8 @@
 """CPU emulation behind the error budget of the decoder's one-plane fp16 operand mode (ops.H1, DESIGN.md section 2).
 
     python tools/decoder_precision_emulation.py [size ...] [--frames noise|smooth]     (default: 256 512, noise)
+    python tools/decoder_precision_emulation.py --stage2 [size ...] [--frames noise|smooth]
+                                                  (stage-2 fast mode; default: 512 1024, smooth and noise; see stage2_main)
 
 The oracle restatement (oracle/restatement.py, torch fp32 on the CPU) is run to the decoder's input (`aligned_volume`), then
 the oracle decoder is run once in exact fp32 and once per operand format with every F.conv2d's input and weights rounded to
@@ -55,7 +57,80 @@ def to_u8(img):
     return (img.clamp(0, 1) * 255).to(torch.uint8)
 
 
+# stage 2 (--stage2): name -> (format of the 7x7 RGB stem, format of every other convolution); None = exact fp32
+STAGE2_FORMATS = {
+    "bf16 x2, stem fp32 (exact mode)": (None, "bf16 x2 (3 MMAs, default)"),
+    "h1, stem fp32": (None, "fp16 x1 scaled (1 MMA, h1)"),
+    "h1, stem h1 too (fast mode)": ("fp16 x1 scaled (1 MMA, h1)", "fp16 x1 scaled (1 MMA, h1)"),
+}
+
+
+def forward(R, sd, img, size):
+    """R.stage2_forward, also returning the latent: (latent, add, ffhq)"""
+    resized = F.interpolate(img, mode="bilinear", size=(size, size), align_corners=False)
+    vol = R.stage2_local_encoder(sd, resized)
+    add = R.stage2_decoder(sd, vol)
+    return vol, add, (resized + add).clamp(min=0, max=1)
+
+
+def stage2_main(sizes, kinds):
+    """Stage-2 fast mode (stage2.Stage2Model(precision="fast")): the oracle stage2_forward, synthetic seed-0 weights, oracle
+    frame 21 (512^2) as the input image, with every F.conv2d of the refinement network evaluated in each STAGE2_FORMATS
+    row.  The stem's operands are rounded as emo_stem_pack and the packed stem weight round them (fp16(16 x), fp16(256 w)).
+    The device folds the pooled 3x3 convolutions into 4x4 stride-2 ones and the up-sampling 3x3 convolutions into sub-pixel
+    2x2 ones before it rounds their weights; the emulation rounds the unfolded weights.  Printed against the fp32 result:
+    ffhq max-abs / mean-abs, PSNR, uint8 pixels changed (trunc(x * 255), the wrapper's conversion), `add` max-abs, the latent's
+    max-abs error and largest magnitude, and the largest |activation| / |weight| any convolution reads."""
+    from emoportraits_b200.stage2 import Stage2Config, synthetic_state_dict_s2
+    from oracle import frames as FR
+    from oracle import restatement as R
+
+    conv2d = F.conv2d
+    for size in sizes:
+        cfg = Stage2Config(output_size=size)
+        sd = synthetic_state_dict_s2(cfg, 0)
+        for kind in kinds:
+            img = FR.frame(512, 21, kind)
+            seen = {"x": 0.0, "w": 0.0}
+
+            def watch(x, w, *a, **k):
+                seen["x"] = max(seen["x"], x.abs().max().item())
+                seen["w"] = max(seen["w"], w.abs().max().item())
+                return conv2d(x, w, *a, **k)
+
+            with torch.no_grad():
+                F.conv2d = watch
+                try:
+                    vol0, add0, ffhq0 = forward(R, sd, img, size)
+                finally:
+                    F.conv2d = conv2d
+                print(f"{size}^2 {kind:6s} largest |activation| into a conv {seen['x']:.2f}, |weight| {seen['w']:.3f}", flush=True)
+                for name, (stem_fmt, fmt) in STAGE2_FORMATS.items():
+                    body = emulated_conv2d(fmt, conv2d)
+                    stem = emulated_conv2d(stem_fmt, conv2d) if stem_fmt else conv2d
+                    F.conv2d = lambda x, w, *a, **k: (stem if w.shape[1] == 3 else body)(x, w, *a, **k)
+                    try:
+                        vol, add, ffhq = forward(R, sd, img, size)
+                    finally:
+                        F.conv2d = conv2d
+                    err = (ffhq - ffhq0).abs()
+                    mse = (err ** 2).mean().item()
+                    psnr = 10 * math.log10(1.0 / mse) if mse > 0 else float("inf")
+                    u8, u80 = (ffhq * 255).to(torch.uint8), (ffhq0 * 255).to(torch.uint8)
+                    changed = (u8 != u80).float().mean().item()
+                    levels = (u8.int() - u80.int()).abs().max().item()
+                    e_vol = (vol - vol0).abs().max().item()
+                    print(f"{size}^2 {kind:6s} {name:32s} ffhq max-abs {err.max().item():.1e} mean-abs {err.mean().item():.1e}  "
+                          f"PSNR {psnr:5.1f} dB  uint8 pixels changed {100 * changed:.2f} % (at most {levels} level)  "
+                          f"add max-abs {(add - add0).abs().max().item():.1e}  latent max-abs {e_vol:.1e} (of max {vol0.abs().max().item():.1f})", flush=True)
+
+
 def main():
+    if "--stage2" in sys.argv:
+        kinds = [sys.argv[sys.argv.index("--frames") + 1]] if "--frames" in sys.argv else ["smooth", "noise"]
+        sizes = [int(a) for a in sys.argv[1:] if a.isdigit()] or [512, 1024]
+        stage2_main(sizes, kinds)
+        return
     args = [a for a in sys.argv[1:] if not a.startswith("--")]
     kind = sys.argv[sys.argv.index("--frames") + 1] if "--frames" in sys.argv else "noise"
     args = [a for a in args if a != kind]

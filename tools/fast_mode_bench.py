@@ -2,6 +2,7 @@
 """Exact vs fast mode (decoder on one fp16 operand plane, ops.H1) in the same run on the same card; one JSON line.
 
     python tools/fast_mode_bench.py [--steps K] [--warmup W] [--rounds R]
+    python tools/fast_mode_bench.py --stage2 [--steps K] [--warmup W] [--rounds R]     (stage 2: see main_stage2)
 
 Per mode, with bench.py's definitions (driver frame @512^2, shipped model, synthetic seed-0 weights, cached source identity):
   fps          device-resident driver frames/s, four captured frames in flight (infer.DriverPipeline depth 4), CUDA events
@@ -159,13 +160,103 @@ def measure(model, st, frames_host, frames_dev, K, W):
     return out
 
 
+def _card():
+    props = torch.cuda.get_device_properties(0)
+    out = {"gpu": props.name, "sm_count": props.multi_processor_count}
+    try:
+        out["power_limit"] = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader"],
+                                            capture_output=True, text=True, timeout=30).stdout.strip()
+    except (OSError, subprocess.SubprocessError):
+        out["power_limit"] = None
+    return out
+
+
+def stage2_images_per_s(model, img, K, W):
+    for _ in range(W):
+        model.forward(img)
+    torch.cuda.synchronize()
+    sampler = bench.ClockSampler(torch.cuda.current_device())
+    sampler.start()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(K):
+        model.forward(img)
+    e1.record()
+    torch.cuda.synchronize()
+    return img.shape[0] * K / (e0.elapsed_time(e1) / 1000.0), sampler.stop()
+
+
+def stage2_times(model, img):
+    """(graph-timed stage-2 convolutions ms per image, per-shape table, stem ms per image: conv_direct, stem_pack + conv_igemm)"""
+    from emoportraits_b200 import ops
+
+    B, S = img.shape[0], model.cfg.output_size
+    prof = ops.ConvProfiler()
+    ops.set_conv_profiler(prof)
+    model.forward(img)
+    torch.cuda.synchronize()
+    ops.set_conv_profiler(None)
+    table, conv_us = [], 0.0
+    for name, n, _ms, _alg, _mma in prof.table():
+        us = graph_time_conv(name)
+        conv_us += us * n
+        table.append({"shape": name, "launches": n, "us_per_launch": us})
+    x4 = ops.resize_bilinear(img, (S, S))
+    stem_h1 = ops.pack_stem_weight(model.stem_w.cpu(), device="cuda")
+    direct_us = _graph_us(lambda: ops.conv_direct(x4, model.stem_w, 1, 3, model.stem_b), 1, replays=20)
+    igemm_us = _graph_us(lambda: ops.conv_igemm(ops.stem_pack(x4), stem_h1, pad=(0, 3, 0), bias=model.stem_b), 1, replays=20)
+    return conv_us / 1000.0 / B, table, {"conv_direct": direct_us / 1000.0 / B, "stem_pack+conv_igemm": igemm_us / 1000.0 / B}
+
+
+def main_stage2(args):
+    """Stage 2 exact vs fast with bench.py's stage-2 definition (@1024^2, batch 4, synthetic seed-0 weights, torch.rand 512^2
+    input): images/s alternated over the rounds, the stage-2 convolutions graph-timed per image (the ConvProfiler's shapes of
+    one forward, each as CUDA-graph replays without its post-op, as decoder_times does), and the 7x7 stem per image both ways."""
+    from emoportraits_b200.stage2 import Stage2Config, Stage2Model, synthetic_state_dict_s2
+
+    cfg = Stage2Config(output_size=1024)
+    sd = synthetic_state_dict_s2(cfg, 0)
+    models = {m: Stage2Model(cfg, sd, "cuda", precision=m) for m in ("exact", "fast")}
+    torch.manual_seed(0)
+    img = torch.rand(4, 3, 512, 512, device="cuda")
+    K, W = args.steps, max(args.warmup, 3)
+    runs = {m: [] for m in models}
+    for _ in range(args.rounds):
+        for m in models:
+            runs[m].append(stage2_images_per_s(models[m], img, K, W))
+    res = {}
+    for m, rs in runs.items():
+        conv_ms, table, stem = stage2_times(models[m], img)
+        res[m] = {"images_per_s": statistics.median(r[0] for r in rs), "images_per_s_runs": [r[0] for r in rs],
+                  "conv_ms_per_image_graph": conv_ms, "conv_shapes": table, "clocks": [r[1] for r in rs]}
+        if m == "exact":
+            res["stem_ms_per_image_graph"] = stem
+    with torch.no_grad():
+        ffhq = {m: models[m].forward(img)[2] for m in models}
+    d = (ffhq["fast"] - ffhq["exact"]).abs()
+    u8 = {m: (ffhq[m] * 255).to(torch.uint8) for m in ffhq}
+    line = {"metric": "stage-2 fast mode (every convolution on one fp16 operand plane, stem on the tensor cores) vs exact, "
+                      "images/s @1024^2 batch 4",
+            **_card(), "steps": K, "warmup": W, "rounds": args.rounds, "exact": res["exact"], "fast": res["fast"],
+            "speedup": res["fast"]["images_per_s"] / res["exact"]["images_per_s"],
+            "conv_speedup_graph": res["exact"]["conv_ms_per_image_graph"] / res["fast"]["conv_ms_per_image_graph"],
+            "stem_ms_per_image_graph": res["stem_ms_per_image_graph"],
+            "ffhq_vs_exact": {"max_abs": d.max().item(), "mean_abs": d.mean().item(),
+                              "uint8_changed": (u8["fast"] != u8["exact"]).float().mean().item()}}
+    print(json.dumps(line))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=200)
     ap.add_argument("--warmup", type=int, default=10)
     ap.add_argument("--rounds", type=int, default=3)
+    ap.add_argument("--stage2", action="store_true", help="the stage-2 arm (main_stage2) instead of the stage-1 decoder's")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "tools/fast_mode_bench.py measures on the GPU"
+    if args.stage2:
+        main_stage2(args)
+        return
     from emoportraits_b200.checkpoint import synthetic_head_pose_state_dict, synthetic_state_dict
     from emoportraits_b200.config import shipped_config
     from emoportraits_b200.infer import Model
