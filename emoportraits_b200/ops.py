@@ -415,8 +415,9 @@ _SPLITK_WS = {}
 
 
 def _splitk_workspace(device) -> torch.Tensor:
-    """Per-device (and per scratch slot, see set_slot) zero-initialised fp32 workspace for split-K convolutions (the
-    finalize kernel leaves it zeroed).  Launches on one stream use it back to back, which is how the model issues its convs."""
+    """Per-device (and per scratch slot, see set_slot) fp32 workspace for split-K convolutions.  It needs no initial state:
+    each K part stores its partial sums to its own slice with plain stores, and the finalize / post kernels read only those
+    slices and write nothing back.  Launches on one stream use it back to back, which is how the model issues its convs."""
     key = (_dev_key(device), _SLOT)
     if key not in _SPLITK_WS:
         _SPLITK_WS[key] = torch.zeros(2 * 1024 * 1024, dtype=torch.float32, device=device)

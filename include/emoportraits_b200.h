@@ -214,9 +214,10 @@ typedef struct {
   /* MMAs accumulated in one wgmma register chunk before it is added to the fp32 sums (0 = default 24).  The tensor core
    * accumulates with truncation; short chunks keep that bias ~1e-6 relative (DESIGN.md "precision"). */
   int acc_chunk_mmas;
-  /* optional split-K workspace: fp32, >= N*Dout*Hout*Wout*Cout elements, ALL ZERO on entry and left all zero on exit.
-   * When given, layers with too few tiles to fill the machine split their K loop over CTAs (partials red.add'ed here,
-   * then one finalize launch applies bias/residual/activation/statistics).  NULL: never split. */
+  /* optional split-K workspace: fp32, >= 2*N*Dout*Hout*Wout*Cout elements, no initial state needed.  When given, layers
+   * with too few tiles to fill the machine split their K loop over CTAs (each part stores its partial sums to its own slice
+   * of N*Dout*Hout*Wout*Cout elements, then one finalize launch sums the slices in part order and applies
+   * bias/residual/activation/statistics; the workspace is not written back).  NULL: never split. */
   float* splitk_ws;
   long long splitk_ws_elems;
   /* sub-pixel evaluation of `nearest x2 -> 3x3 conv` (ImageDecoder up blocks, decoder.py:241-358 / utils.py:761-788 with

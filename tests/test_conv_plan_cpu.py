@@ -140,61 +140,40 @@ def test_case_table_reaches_every_configuration(plans):
     assert not missing, f"configurations no case of tests/conv_plan_cases.py reaches: {missing}"
 
 
-CATALOGUE = r"""
-import ctypes as C, json, sys
-sys.path.insert(0, %r)
-import torch
-from emoportraits_b200 import lib as L
-assert L.DRY_RUN
-lib = L.load()
-rows = {}
-launch = L.call
-def call(name, *args):
-    if name == "emo_conv_igemm":
-        d = args[0]._obj
-        info = L.ConvPlanInfo()
-        rc = lib.emo_conv_plan(C.byref(d), 132, C.byref(info))
-        key = "%%dx%%dx%%dx%%dx%%d->%%d k%%d%%d%%d s%%d%%s%%s" %% (d.N, d.Din, d.Hin, d.Win, d.Cin, d.Cout, d.kd, d.kh, d.kw, d.sh,
-              " up2" if d.upconv else "", " post" if d.post else "")
-        rows[key] = dict(rc=rc, err=lib.emo_last_error().decode() if rc else "", info={f: getattr(info, f) for f, _ in info._fields_})
-    return launch(name, *args)
-L.call = call
-which = sys.argv[1]
-if which.startswith("s1"):
-    from emoportraits_b200.checkpoint import synthetic_head_pose_state_dict, synthetic_state_dict
-    from emoportraits_b200.config import shipped_config
-    from emoportraits_b200.infer import Model
-    size = int(which[3:])
-    cfg = shipped_config(size)
-    model = Model(cfg, synthetic_state_dict(cfg, 0), synthetic_head_pose_state_dict(0), "cpu")
-    x = torch.rand(1, 3, size, size)
-    model.driver_pass(model.source_pass(x), x, mix=True)
-else:
-    from emoportraits_b200.stage2 import Stage2Config, Stage2Model, synthetic_state_dict_s2
-    cfg = Stage2Config(output_size=int(which[3:]))
-    Stage2Model(cfg, synthetic_state_dict_s2(cfg, 0), "cpu").forward(torch.rand(1, 3, 512, 512))
-print("CATALOGUE " + json.dumps(rows))
-"""
+def _old_key(rec):
+    """the shape key this test used to file launches under: it left out res_shift, pads, strides other than sh, the operand
+    planes and which optional pointers are set, so launches differing only there overwrote each other"""
+    d = rec["conv"]
+    return "%dx%dx%dx%dx%d->%d k%d%d%d s%d%s%s" % (d["N"], d["Din"], d["Hin"], d["Win"], d["Cin"], d["Cout"], d["kd"], d["kh"],
+                                               d["kw"], d["sh"], " up2" if d["upconv"] else "", " post" if rec["post"] else "")
 
 
 @pytest.mark.parametrize("model", ["s1-256", "s1-512", "s2-512", "s2-1024"])
 def test_model_layers_fall_in_swept_plan_classes(model):
+    """every distinct launch (tests/model_conv_launches.py's full record) of the exact-mode model; stage 2 at batch 1"""
     from emoportraits_b200 import lib as L
 
+    config = model + ("-exact" if model.startswith("s1") else "-b1-exact")
     env = dict(os.environ, EMO_DRY_RUN="1")
-    r = subprocess.run([sys.executable, "-c", CATALOGUE % str(ROOT), model], env=env, capture_output=True, text=True, timeout=900)
+    r = subprocess.run([sys.executable, str(ROOT / "tests" / "model_conv_launches.py"), config], env=env, capture_output=True,
+                       text=True, timeout=900)
     assert r.returncode == 0, r.stdout + r.stderr
-    rows = json.loads(r.stdout.split("CATALOGUE ", 1)[1])
+    rows = json.loads(r.stdout.split("LAUNCHES ", 1)[1])
     assert rows, "no emo_conv_igemm call recorded"
-    refused = {k: v["err"] for k, v in rows.items() if v["rc"] != 0}
+    refused = [(_old_key(v), v["err"]) for v in rows if v["rc"] != 0]
     assert not refused, refused
     swept = {c.want for c in CP.CASES}
-    print(f"\n[{model} conv layers: plan class at 132 SMs]")
+    old = {_old_key(v) for v in rows}
+    print(f"\n[{model} conv layers: plan class at 132 SMs] {len(rows)} distinct launches; the shape key alone would merge "
+          f"{len(rows) - len(old)} of them into others")
     unswept = []
-    for key, v in sorted(rows.items()):
-        info = L.ConvPlanInfo(**v["info"])
+    for v in rows:
+        d = v["conv"]
+        info = L.ConvPlanInfo(**v["plan"])
         cls = CP.plan_class(info)
-        print(f"  {key:44s} {cls:36s} ksplit {info.ksplit:2d} grid {info.grid:3d}")
+        opts = " ".join(sorted(set(v["conv_ptrs"]) - {"a_hi", "a_lo", "a_lo2", "w_hi", "w_lo", "w_lo2", "out", "splitk_ws"}))
+        name = f"{_old_key(v)} p{d['ph']}{d['pw']} rs{d['res_shift']} act{d['act']} [{opts}]"
+        print(f"  {name:90s} {cls:36s} ksplit {info.ksplit:2d} grid {info.grid:3d}")
         if cls not in swept:
-            unswept.append((key, cls))
+            unswept.append((name, cls))
     assert not unswept, f"model layers in plan classes no case of tests/conv_plan_cases.py checks: {unswept}"

@@ -104,6 +104,18 @@ CASES = [
     ("h1<32,1> BN96 tap none", CP.Case("", 160, 96, (96, 96), k=1, planes=H1)),
     ("h1ps<64,1> BN128 rr3 none", CP.Case("", 128, 128, (64, 64), planes=H1, upconv=True, stats=True)),
     ("h1ps<64,1> BN64 rr3 none", CP.Case("", 256, 64, (48, 40), planes=H1, upconv=True, residual=True, res_shift=1, stats=True)),
+    # the 160 / 320 and 96 / 192 channel layers of the 256^2 / 512^2 decoders
+    ("h1<64,1> BN80 rr3 none", CP.Case("", 64, 160, (96, 40), planes=H1, residual=True, stats=True)),
+    ("h1<64,1> BN80 rr3 apply", CP.Case("", 64, 160, (96, 40), planes=H1, post=True, stats=True)),
+    ("h1<64,1> BN80 tap none", CP.Case("", 64, 160, (96, 40), k=1, planes=H1)),
+    ("h1<64,1> BN96 rr3 none", CP.Case("", 64, 192, (96, 40), planes=H1, residual=True)),
+    ("h1<64,1> BN96 rr3 apply", CP.Case("", 64, 192, (96, 40), planes=H1, post=True, stats=True)),
+    ("h1<64,1> BN96 tap none", CP.Case("", 64, 192, (96, 40), k=1, planes=H1, stats=True)),
+    ("h1<32,1> BN80 rr3 none", CP.Case("", 160, 160, (96, 40), planes=H1, residual=True, stats=True)),
+    ("h1<32,1> BN80 rr3 apply", CP.Case("", 32, 160, (96, 40), planes=H1, post=True, stats=True)),
+    ("h1<32,1> BN96 rr3 apply", CP.Case("", 160, 96, (96, 96), planes=H1, post=True, stats=True)),
+    ("h1ps<64,1> BN80 rr3 none", CP.Case("", 64, 160, (24, 40), planes=H1, upconv=True, residual=True, stats=True)),
+    ("h1ps<64,1> BN96 rr3 none", CP.Case("", 64, 96, (48, 48), planes=H1, upconv=True, residual=True, res_shift=1)),
 ]
 
 
