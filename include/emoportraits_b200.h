@@ -391,7 +391,8 @@ int emo_split_f16(const float* x, long long n, float scale, void* hi, void* lo, 
  *   emo_u8_to_image   uint8 [N][H][W][C] (PIL / numpy layout) -> fp32 [N][C][H][W] = u / 255
  *                     replaces transforms.ToTensor() in notebooks/infer.py:229-243 (convert_to_tensor)
  *   emo_image_to_u8   fp32 [N][C][H][W] -> uint8 [N][H][W][C] = trunc(clamp(x, 0, 1) * 255)
- *                     replaces `.clamp(0, 1)` + transforms.ToPILImage() (mul(255).byte()) notebooks/infer.py:641-644
+ *                     replaces `.clamp(0, 1)` + transforms.ToPILImage() (mul(255).byte()) notebooks/infer.py:641-644;
+ *                     a NaN pixel becomes 0 (torch's clamp keeps the NaN, whose byte conversion is undefined)
  *   emo_resize_bicubic fp32 [N][C][Hin][Win] -> [N][C][Hout][Wout]: F.interpolate(mode='bicubic', align_corners=False),
  *                     A = -0.75, border-replicated taps; replaces notebooks/infer.py:399-403, 551-556
  * ------------------------------------------------------------------------------------------------ */

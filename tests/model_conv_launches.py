@@ -58,20 +58,17 @@ def key(rec: dict) -> str:
     return json.dumps({k: v for k, v in rec.items() if k != "configs"}, sort_keys=True)
 
 
-def record(config: str) -> list:
-    """the records of every emo_conv_igemm call of one configuration, in launch order (needs lib.DRY_RUN)"""
+def run(config: str, hook) -> None:
+    """run the models of one configuration in EMO_DRY_RUN mode, calling hook(name, *args) before every C-ABI call"""
     import torch
 
     from emoportraits_b200 import lib as L
 
-    assert L.DRY_RUN, "record() runs the models in EMO_DRY_RUN mode"
-    lib = L.load()
-    recs = []
+    assert L.DRY_RUN, "the models are recorded in EMO_DRY_RUN mode"
     launch = L.call
 
     def call(name, *args):
-        if name == "emo_conv_igemm":
-            recs.append(launch_record(L, lib, args[0]._obj))
+        hook(name, *args)
         return launch(name, *args)
 
     stage, size, *rest = config.split("-")
@@ -96,6 +93,20 @@ def record(config: str) -> list:
             model.forward(torch.rand(int(rest[0][1:]), 3, 512, 512))
     finally:
         L.call = launch
+
+
+def record(config: str) -> list:
+    """the records of every emo_conv_igemm call of one configuration, in launch order (needs lib.DRY_RUN)"""
+    from emoportraits_b200 import lib as L
+
+    lib = L.load()
+    recs = []
+
+    def hook(name, *args):
+        if name == "emo_conv_igemm":
+            recs.append(launch_record(L, lib, args[0]._obj))
+
+    run(config, hook)
     return recs
 
 

@@ -55,17 +55,43 @@ def cdiv(a, b):
 # ------------------------------------------------------------------------------------------------------------------
 # host restatement of the dispatch
 # ------------------------------------------------------------------------------------------------------------------
+# the arguments of the entry points that take them positionally (the trailing stream excluded)
+POSITIONAL = {"emo_gn_stats": ("x", "N", "S", "C", "G", "stats"),
+              "emo_maxpool2d_3x3s2": ("x", "N", "H", "W", "C", "out"),
+              "emo_global_avgpool": ("x", "N", "S", "C", "out"),
+              "emo_split_bf16": ("x", "n", "hi", "lo", "lo2"),
+              "emo_split_f16": ("x", "n", "scale", "hi", "lo"),
+              "emo_stem_pack": ("x", "N", "H", "W", "C", "scale", "out"),
+              "emo_u8_to_image": ("x", "N", "H", "W", "C", "out"),
+              "emo_image_to_u8": ("x", "N", "C", "H", "W", "out"),
+              "emo_resize_bicubic": ("x", "N", "C", "Hin", "Win", "Hout", "Wout", "out"),
+              "emo_composite": ("img", "mask", "bg", "N", "C", "H", "W", "threshold", "out"),
+              "emo_parsing_prepare": ("x", "N", "C", "Hin", "Win", "Hout", "Wout", "mean", "std", "out"),
+              "emo_parsing_masks": ("x", "N", "K", "Hin", "Win", "Hout", "Wout", "label_sets", "out", "labels"),
+              "emo_resize_area": ("x", "N", "C", "Hin", "Win", "Hout", "Wout", "scale", "shift", "out")}
+# which of them are device pointers (label_sets is a host array of four class bit sets: a scalar argument)
+POSITIONAL_POINTERS = {"x", "stats", "out", "hi", "lo", "lo2", "img", "mask", "bg", "mean", "std", "labels"}
+
+
 def fields(name: str, args) -> dict:
     """the arguments of one C-ABI call as {field: value}; pointers are ints (0 for NULL)"""
     if args and hasattr(args[0], "_obj"):
         d = args[0]._obj
         return {f: (getattr(d, f) or 0) if t is C.c_void_p else getattr(d, f) for f, t in d._fields_}
-    names = {"emo_gn_stats": ("x", "N", "S", "C", "G", "stats"),
-             "emo_maxpool2d_3x3s2": ("x", "N", "H", "W", "C", "out"),
-             "emo_global_avgpool": ("x", "N", "S", "C", "out"),
-             "emo_split_bf16": ("x", "n", "hi", "lo", "lo2"),
-             "emo_split_f16": ("x", "n", "scale", "hi", "lo")}[name]
-    return {k: (v.value if hasattr(v, "value") else v) or 0 for k, v in zip(names, args)}
+    out = {}
+    for k, v in zip(POSITIONAL[name], args):
+        if isinstance(v, C.Array):
+            out[k] = list(v)
+        else:
+            out[k] = (v.value if hasattr(v, "value") else v) or 0
+    return out
+
+
+def pointer_fields(name: str, args) -> set:
+    """the names of the pointer arguments of one C-ABI call (NULL or not)"""
+    if args and hasattr(args[0], "_obj"):
+        return {f for f, t in args[0]._obj._fields_ if t is C.c_void_p}
+    return set(POSITIONAL[name]) & POSITIONAL_POINTERS
 
 
 def _outs(f, fp16_key="plane_fp16"):
@@ -223,7 +249,31 @@ def classify(name: str, f: dict):
     if op in ("split_bf16", "split_f16"):
         n = (3 if f["lo2"] else 2) if op == "split_bf16" else (2 if f["lo"] else 1)
         return f"{op} x{n}", {f"{op} x{n}"}
+    if op == "stem_pack":
+        feats.add("stem_pack")
+        if f["N"] * f["H"] * f["W"] > STRIDE_CAP * 256:
+            feats.add("stem_pack grid-stride loop")
+        return op, feats
+    if op in BOUNDARY_GRID:
+        # the wrapper-boundary kernels (tests/model_op_launches.py BOUNDARY): capped grid-stride loops
+        work = {"u8_to_image": ("N", "H", "W"), "image_to_u8": ("N", "H", "W"), "composite": ("N", "C", "H", "W"),
+                "resize_bicubic": ("N", "C", "Hout", "Wout"), "parsing_prepare": ("N", "C", "Hout", "Wout"),
+                "parsing_masks": ("N", "Hout", "Wout"), "resize_area": ("N", "C", "Hout", "Wout")}[op]
+        blocks, threads = BOUNDARY_GRID[op]
+        if math.prod(f[k] for k in work) > blocks * threads:
+            feats.add(f"{op} grid-stride loop")
+        if "Hin" in f:
+            hi, wi, ho, wo = f["Hin"], f["Win"], f["Hout"], f["Wout"]
+            feats.add(f"{op} {'same size' if (hi, wi) == (ho, wo) else 'up' if ho > hi or wo > wi else 'down'}")
+        return op, feats
     raise KeyError(name)
+
+
+STRIDE_CAP = SM_COUNT * 16   # CTAs of the capped grid-stride loops (emo_stem_pack, the image conversions, the composite)
+# (CTAs, threads per CTA) of each wrapper-boundary kernel's capped grid
+BOUNDARY_GRID = {"u8_to_image": (STRIDE_CAP, 256), "image_to_u8": (STRIDE_CAP, 256), "composite": (STRIDE_CAP, 256),
+                 "resize_bicubic": (STRIDE_CAP, 256), "parsing_prepare": (STRIDE_CAP, 256),
+                 "parsing_masks": (SM_COUNT * 32, 128), "resize_area": (STRIDE_CAP, 256)}
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -345,12 +395,16 @@ CASES += [
     case("split_bf16", "split_bf16 x3", n=4 * 10007, planes=3),
     case("split_f16", "split_f16 x2", n=4 * 10007, planes=2),
     case("split_f16", "split_f16 x1", n=4 * 10007, planes=1),
+    # ---- emo_stem_pack: one pass, and the capped grid's stride loop (768 x 720 pixels > 2112 CTAs x 256) ----
+    case("stem_pack", "stem_pack", N=2, H=37, W=53),
+    case("stem_pack", "stem_pack", N=1, H=768, W=720),
 ]
 
 
-# C-ABI entry points outside the table: the convolution (tests/conv_plan_cases.py), the mask kernels (tests/test_masks.py),
-# the pose algebra (tests/test_pose_math_host.py), the wrapper-boundary image conversions (tests/test_ops_gpu.py) and the
-# benchmark's L2 flush
+# C-ABI entry points outside the table: the convolution (tests/conv_plan_cases.py), the pose algebra
+# (tests/test_pose_math_host.py), the wrapper-boundary image conversions and mask kernels (tests/test_ops_gpu.py,
+# tests/test_masks.py, and at the wrappers' shapes the BOUNDARY launches of tests/model_op_launches.py) and the benchmark's
+# L2 flush
 NOT_IN_TABLE = ("conv_igemm", "pose_theta", "u8_to_image", "image_to_u8", "resize_bicubic", "composite", "parsing_prepare",
                 "parsing_masks", "resize_area", "l2_flush", "l2_flush_clean")
 
@@ -394,6 +448,7 @@ def required() -> list:
     req += ["H odd", "H even", "W odd", "W even", "all-negative input", "S >= 256^2"]
     req += ["same size", "up", "down", "non-integer ratio", "C_pad > C zero fill", "mean/std", "lattice partly outside", "NCHW copy"]
     req += ["split_bf16 x2", "split_bf16 x3", "split_f16 x2", "split_f16 x1"]
+    req += ["stem_pack", "stem_pack grid-stride loop"]
     return req
 
 
@@ -514,6 +569,10 @@ def inputs(c: Case, device) -> dict:
         x = torch.randn(k["n"], generator=g) * torch.exp2(torch.randint(-12, 10, (k["n"],), generator=g).float())
         x[:4] = torch.tensor([0.0, -0.0, 3.0e-8, 1000.0])
         t["x"] = x
+    elif c.op == "stem_pack":
+        x = torch.zeros(k["N"], 1, k["H"], k["W"], 4)
+        x[..., :3] = (torch.randn(k["N"], 1, k["H"], k["W"], 3, generator=g) * 1.5).clamp(-2.2, 2.7)   # normalised RGB
+        t["x"] = x
     return {n: (v.to(device) if isinstance(v, torch.Tensor) else v) for n, v in t.items()}
 
 
@@ -569,6 +628,8 @@ def out_specs(c: Case) -> dict:
         return o
     if c.op in ("split_bf16", "split_f16"):
         return {"planes": ((k["planes"], k["n"]), torch.bfloat16 if c.op == "split_bf16" else torch.float16)}
+    if c.op == "stem_pack":
+        return {"out": ((k["N"], 1, k["H"], k["W"], 32), torch.float16)}
     raise KeyError(c.op)
 
 
@@ -645,6 +706,8 @@ def launch(c: Case, ops, t: dict, o: dict):
         return name, (p(t["x"]), k["n"], pp[0], pp[1], pp[2], ops._stream())
     if c.op == "split_f16":
         return name, (p(t["x"]), k["n"], C.c_float(F16_SCALE), pp[0], pp[1], ops._stream())
+    if c.op == "stem_pack":
+        return name, (p(t["x"]), k["N"], k["H"], k["W"], 4, C.c_float(F16_SCALE), p(o["out"]), ops._stream())
     raise KeyError(c.op)
 
 

@@ -1,14 +1,10 @@
 """CPU tests of the non-convolution case table (tests/op_cases.py):
   * every case reaches the kernel variant it names (the host restatement of its entry point's dispatch);
   * the table as a whole reaches every variant: a variant no case reaches fails here, by name;
-  * every non-convolution launch the shipped models issue (stage 1 at 256 and 512, stage 2 at 512 and 1024, recorded in
-    EMO_DRY_RUN mode), and the post-op of every convolution, falls in a variant class of the table;
+  * (tests/test_model_op_launches_cpu.py) every non-convolution launch the shipped models issue, and the post-op of every
+    convolution, falls in a variant class of the table;
   * the GroupNorm inputs of the models stay within the mean/std range tests/test_op_cases_gpu.py asserts its bar over."""
-import json
-import os
 import pathlib
-import subprocess
-import sys
 
 import pytest
 import torch
@@ -60,66 +56,6 @@ def test_case_table_reaches_every_variant(classified):
         print(f"  {r:40s} {len(reached.get(r, [])):3d}  {reached.get(r, ['-'])[0]}")
     missing = [r for r in req if r not in reached]
     assert not missing, f"variants no case of tests/op_cases.py reaches: {missing}"
-
-
-CATALOGUE = r"""
-import ctypes as C, json, sys
-sys.path.insert(0, %r)
-sys.path.insert(0, %r)
-import torch
-from emoportraits_b200 import lib as L
-import op_cases as OC
-assert L.DRY_RUN
-rows = {}
-launch = L.call
-def call(name, *args):
-    if name == "emo_conv_igemm":
-        post = args[0]._obj.post
-        if post:
-            d = C.cast(post, C.POINTER(L.ApplyDesc)).contents
-            cls, _ = OC.classify("emo_apply", OC.fields("emo_apply", (C.byref(d),)))
-            rows.setdefault("conv post-op: " + cls, 0)
-            rows["conv post-op: " + cls] += 1
-    elif name[4:] not in OC.NOT_IN_TABLE:
-        cls, _ = OC.classify(name, OC.fields(name, args))
-        rows.setdefault(cls, 0)
-        rows[cls] += 1
-    return launch(name, *args)
-L.call = call
-which = sys.argv[1]
-if which.startswith("s1"):
-    from emoportraits_b200.checkpoint import synthetic_head_pose_state_dict, synthetic_state_dict
-    from emoportraits_b200.config import shipped_config
-    from emoportraits_b200.infer import Model
-    size = int(which[3:])
-    cfg = shipped_config(size)
-    model = Model(cfg, synthetic_state_dict(cfg, 0), synthetic_head_pose_state_dict(0), "cpu")
-    x = torch.rand(1, 3, size, size)
-    model.driver_pass(model.source_pass(x), x, mix=True)
-else:
-    from emoportraits_b200.stage2 import Stage2Config, Stage2Model, synthetic_state_dict_s2
-    cfg = Stage2Config(output_size=int(which[3:]))
-    Stage2Model(cfg, synthetic_state_dict_s2(cfg, 0), "cpu").forward(torch.rand(1, 3, 512, 512))
-print("CATALOGUE " + json.dumps(rows))
-"""
-
-@pytest.mark.parametrize("model", ["s1-256", "s1-512", "s2-512", "s2-1024"])
-def test_model_launches_fall_in_table_variants(model):
-    env = dict(os.environ, EMO_DRY_RUN="1")
-    r = subprocess.run([sys.executable, "-c", CATALOGUE % (str(ROOT), str(ROOT / "tests")), model], env=env, capture_output=True,
-                       text=True, timeout=900)
-    assert r.returncode == 0, r.stdout + r.stderr
-    rows = json.loads(r.stdout.split("CATALOGUE ", 1)[1])
-    assert rows, "no launch recorded"
-    covered = {c.want for c in OC.CASES}
-    print(f"\n[{model} non-convolution launches: variant class]")
-    uncovered = []
-    for cls, n in sorted(rows.items()):
-        base = cls.split(": ", 1)[-1]
-        print(f"  {n:4d}  {cls}")
-        if base not in covered:
-            uncovered.append(cls)
-    assert not uncovered, f"model launches in variants no case of tests/op_cases.py checks: {uncovered}"
 
 
 def test_model_groupnorm_inputs_stay_near_zero_mean():
