@@ -40,6 +40,13 @@ class Model:
     # product instead of three).  Fast mode keeps every uint8 output pixel within one level of the exact path
     # (tools/decoder_precision_emulation.py, tests/test_fast_decoder_gpu.py; INTEGRATION.md "Fast mode").
     PRESETS = dict(exact={}, fast=dict(decoder=ops.H1))
+    # The source-volume networks on one fp16 plane (InferenceWrapper(source_precision="fast")).  Their output is the latent
+    # volume's values, which the sampler and the decoder treat linearly or contract: the same error size as the decoder's fast
+    # mode (tools/decoder_precision_emulation.py --source; DESIGN.md section 2).  The source volume is cached for a whole clip,
+    # so its error is a fixed bias in every frame: this is a setting of its own, not part of PRESETS["fast"].
+    SOURCE_FAST = dict(local_encoder=ops.H1, volume_source=ops.H1, unet3d=ops.H1)
+    # networks whose output feeds the sampler's coordinates: never on one plane
+    SAMPLER_NETS = ("head_pose", "expression", "idt", "warp")
 
     @classmethod
     def resolve_precision(cls, precision) -> dict:
@@ -53,14 +60,15 @@ class Model:
         if pr["decoder"] == ops.H2:
             raise ValueError("the decoder's input planes are written by grid_sample_3d in bf16 or as one fp16 plane; it runs "
                              "with 2 or 3 bf16 planes or ops.H1")
-        one_plane = sorted(net for net, planes in pr.items() if planes == ops.H1 and net != "decoder")
+        one_plane = sorted(net for net in cls.SAMPLER_NETS if pr[net] == ops.H1)
         if one_plane:
-            raise ValueError(f"ops.H1 (one fp16 plane) is for the decoder only, not {one_plane}: the embedding and warp networks "
-                             "feed the sampler, which amplifies their errors ~100x (DESIGN.md section 2)")
+            raise ValueError(f"ops.H1 (one fp16 plane) is not for {one_plane}: the head-pose, expression, identity and warp "
+                             "networks feed the sampler's coordinates, which amplify their errors ~100x (DESIGN.md section 2)")
         return pr
 
     def __init__(self, cfg: HotPathConfig, state_dict, head_pose_state_dict, device="cuda", precision=None):
-        """precision: None / "exact" (PRECISION), "fast" (decoder on ops.H1), or a dict overriding PRECISION per network."""
+        """precision: None / "exact" (PRECISION), "fast" (decoder on ops.H1), or a dict overriding PRECISION per network
+        (SOURCE_FAST puts the local encoder, the source volume blocks and the 3-D U-Net on ops.H1)."""
         self.cfg = cfg
         dev = torch.device(device)
         sd = state_dict
@@ -271,13 +279,19 @@ class InferenceWrapper(torch.nn.Module):
     def __init__(self, experiment_name, which_epoch='latest', model_file_name='', use_gpu=True, num_gpus=1,
                  fixed_bounding_box=False, project_dir='./', folder='mp_logs', model_='va',
                  torch_home='', debug=False, print_model=False, print_params=True, args_overwrite={}, state_dict=None,
-                 pose_momentum=0.5, rank=0, args_path=None, head_pose_state_dict=None, precision="exact"):
+                 pose_momentum=0.5, rank=0, args_path=None, head_pose_state_dict=None, precision="exact",
+                 source_precision="exact"):
         """precision: "exact" (default: the parity path) or "fast" (the decoder on one fp16 plane: every uint8 output pixel
         within one level of "exact", INTEGRATION.md "Fast mode").  Every driver path (captured pipelines, the list form of
-        forward, video.drive_image_with_video) runs with the model's setting."""
+        forward, video.drive_image_with_video) runs with the model's setting.
+        source_precision: "exact" (default) or "fast" (the source pass's local encoder, volume blocks and 3-D U-Net on one
+        fp16 plane, Model.SOURCE_FAST; every uint8 pixel within one level of "exact").  Independent of `precision=`: the
+        source volume is cached, so its error is the same in every frame of a clip."""
         super().__init__()
         if precision not in ("exact", "fast"):
             raise ValueError(f"precision={precision!r}: 'exact' or 'fast'")
+        if source_precision not in ("exact", "fast"):
+            raise ValueError(f"source_precision={source_precision!r}: 'exact' or 'fast'")
         if not use_gpu or not torch.cuda.is_available():
             raise RuntimeError("emoportraits_b200.InferenceWrapper needs a CUDA device (H100); there is no CPU path")
         if model_ != 'va':
@@ -300,8 +314,11 @@ class InferenceWrapper(torch.nn.Module):
             if not hp or not pathlib.Path(str(hp)).exists():
                 raise FileNotFoundError(f"head pose regressor checkpoint not found ({hp}); pass head_pose_state_dict=")
             head_pose_state_dict = torch.load(hp, map_location='cpu')
-        self.precision = precision
-        self.model = Model(self.cfg, state_dict, head_pose_state_dict, self.device, precision=precision)
+        self.precision, self.source_precision = precision, source_precision
+        model_precision = precision
+        if source_precision == "fast":
+            model_precision = dict(Model.PRESETS[precision], **Model.SOURCE_FAST)
+        self.model = Model(self.cfg, state_dict, head_pose_state_dict, self.device, precision=model_precision)
         if rank == 0 and print_params:
             n = sum(v.numel() for v in state_dict.values())
             print(f'Number of parameters/buffers in checkpoint: {n}')

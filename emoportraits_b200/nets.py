@@ -154,6 +154,8 @@ class LocalEncoder:
         p = "local_encoder_nw"
         s = cfg.image_size
         self.stem_w, self.stem_b = stem_weight(sd, f"{p}.from_rgb_{s}px", dev)
+        # one fp16 plane: the stem runs on the tensor cores as a 7x1 implicit GEMM over ops.stem_pack's 32 channels
+        self.stem_h1 = ops.pack_stem_weight(self.stem_w.cpu(), device=dev) if planes == ops.H1 else None
         self.blocks = []
         for i in range(len(cfg.enc_channels) - 1):
             self.blocks.append(ResBlock(sd, f"{p}.enc_{i}_block={s}px", dev, planes=planes, pool_fold=True))
@@ -170,7 +172,10 @@ class LocalEncoder:
         cfg = self.cfg
         x4 = ops.resize_bilinear(img_nchw, img_nchw.shape[-2:])  # same-size bilinear == exact NCHW -> NHWC4 repack
         st = ops.new_stats(1, G, x4.device)
-        x = ops.conv_direct(x4, self.stem_w, 1, 3, self.stem_b, stats=st)
+        if self.stem_h1 is not None:
+            x = ops.conv_igemm(ops.stem_pack(x4), self.stem_h1, pad=(0, 3, 0), bias=self.stem_b, stats=st)
+        else:
+            x = ops.conv_direct(x4, self.stem_w, 1, 3, self.stem_b, stats=st)
         for blk in self.blocks:
             x, st = blk(x, st, down=(1, 2, 2))
         a = ops.apply(x, gn=self.fin_norm.gn(st, _count(x)), act=ops.ACT_RELU, planes=self.planes)

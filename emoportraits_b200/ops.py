@@ -42,8 +42,9 @@ H2 = "h2"
 F16_ACT_SCALE = 16.0    # activations: post-GroupNorm / ReLU values are O(1)
 F16_W_SCALE = 256.0     # spectral-norm / weight-standardised weights are O(0.01 .. 1)
 # fp16 one-plane operand mode ("h1"): ONE fp16 plane of (value * the same power of two as "h2"), one MMA per product instead of
-# three, ~2^-11 relative per operand.  Stage 1's decoder and stage 2 only, in their fast modes (DESIGN.md section 2): the embedding
-# / warp networks feed the sampler, which amplifies their errors ~100x (tools/decoder_precision_emulation.py gives the bounds).
+# three, ~2^-11 relative per operand.  Stage 1's decoder, its source-volume networks (local encoder, volume blocks, 3-D U-Net) and
+# stage 2 only, in their fast modes (DESIGN.md section 2): the embedding / warp networks feed the sampler, which amplifies their
+# errors ~100x (tools/decoder_precision_emulation.py gives the bounds).
 H1 = "h1"
 
 

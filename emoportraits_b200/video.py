@@ -56,7 +56,8 @@ def drive_image_with_video(inferer, source, frames: Sequence, inferer_s2=None, b
     crop_box = (left, upper, right, lower) on the output: the fixed crop of cell 46 (first-frame face box, computed by the
     caller's face detector).
     Each wrapper runs with the `precision=` it was built with: a stage-2 wrapper built with precision="fast" refines every
-    chunk in fast mode, exactly as calling that wrapper on the same chunk would."""
+    chunk in fast mode, exactly as calling that wrapper on the same chunk would.  A stage-1 wrapper built with
+    source_precision="fast" runs the one source pass in fast mode, and every frame reads that cached source volume."""
     from PIL import Image
 
     kw = dict(crop=False, smooth_pose=False, target_theta=True, mix=True, mix_old=False, modnet_mask=False)

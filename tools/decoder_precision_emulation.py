@@ -3,6 +3,9 @@
     python tools/decoder_precision_emulation.py [size ...] [--frames noise|smooth]     (default: 256 512, noise)
     python tools/decoder_precision_emulation.py --stage2 [size ...] [--frames noise|smooth]
                                                   (stage-2 fast mode; default: 512 1024, smooth and noise; see stage2_main)
+    python tools/decoder_precision_emulation.py --source [size ...] [--frames noise|smooth]
+                                                  (source-pass fast mode, alone and with the decoder's; default: 256 512,
+                                                   smooth and noise; see source_main)
 
 The oracle restatement (oracle/restatement.py, torch fp32 on the CPU) is run to the decoder's input (`aligned_volume`), then
 the oracle decoder is run once in exact fp32 and once per operand format with every F.conv2d's input and weights rounded to
@@ -125,7 +128,110 @@ def stage2_main(sizes, kinds):
                           f"add max-abs {(add - add0).abs().max().item():.1e}  latent max-abs {e_vol:.1e} (of max {vol0.abs().max().item():.1f})", flush=True)
 
 
+# source pass (--source): name -> (format of the local encoder / volume blocks / 3-D U-Net convolutions, of the decoder's)
+H1_FMT = "fp16 x1 scaled (1 MMA, h1)"
+SOURCE_FORMATS = {
+    "source h1 (source_precision=fast)": (H1_FMT, None),
+    "decoder h1 (precision=fast)": (None, H1_FMT),
+    "source h1 + decoder h1 (both fast)": (H1_FMT, H1_FMT),
+}
+
+
+def source_main(sizes, kinds):
+    """Source-pass fast mode (InferenceWrapper(source_precision="fast")): the oracle source pass (synthetic seed-0 weights,
+    oracle frame 21) and driver pass (frame 22), with every F.conv2d / F.conv3d of local_encoder, volume_source and unet3d
+    evaluated on one fp16 plane, fp16(16 x) and fp16(256 w), products summed in fp64; the 7x7 RGB stem is rounded the same
+    way (emo_stem_pack and the packed stem weight round it so).  Everything else runs in exact fp32.  The device folds the
+    pooled 3x3 convolutions into 4x4 stride-2 ones before it rounds their weights; the emulation rounds the unfolded weights.
+    Rows: the source networks alone, the decoder alone (precision="fast", for comparison) and both together; the decoder's
+    128 -> 3 image head stays in fp32, as ops.gn_head keeps it on the device.  Printed against the fp32 result: image max-abs
+    / mean-abs, PSNR, uint8 pixels moved (trunc(clamp(x, 0, 1) * 255), the wrapper's conversion) and the largest move,
+    `target_latent_volume` max-abs error (of its largest magnitude), and the largest |activation| / |weight| any source
+    convolution reads."""
+    from emoportraits_b200.checkpoint import synthetic_head_pose_state_dict, synthetic_state_dict
+    from emoportraits_b200.config import shipped_config
+    from oracle import frames as FR
+    from oracle import restatement as R
+
+    conv2d, conv3d = F.conv2d, F.conv3d
+    nets = {name: getattr(R, name) for name in ("local_encoder", "volume_source", "unet3d", "decoder")}
+    where = [None]      # the oracle network being evaluated
+
+    def scoped(name):
+        def run(*a, **k):
+            where[0] = name
+            try:
+                return nets[name](*a, **k)
+            finally:
+                where[0] = None
+        return run
+
+    def install(src_fmt, dec_fmt, seen=None):
+        def pick(base):
+            src = emulated_conv2d(src_fmt, base) if src_fmt else base
+            dec = emulated_conv2d(dec_fmt, base) if dec_fmt else base
+
+            def conv(x, w, *a, **k):
+                if where[0] == "decoder":
+                    return (dec if w.shape[0] > 4 else base)(x, w, *a, **k)     # the image head stays fp32 (ops.gn_head)
+                if where[0] is not None:
+                    if seen is not None:
+                        seen["x"] = max(seen["x"], x.abs().max().item())
+                        seen["w"] = max(seen["w"], w.abs().max().item())
+                    return src(x, w, *a, **k)
+                return base(x, w, *a, **k)
+            return conv
+        F.conv2d, F.conv3d = pick(conv2d), pick(conv3d)
+
+    for name in nets:
+        setattr(R, name, scoped(name))
+    try:
+        for size in sizes:
+            cfg = shipped_config(size)
+            sd, hsd = synthetic_state_dict(cfg, 0), synthetic_head_pose_state_dict(0)
+            ocfg = R.config_from_state_dict(sd, size)
+            for kind in kinds:
+                src, drv = FR.frame(size, 21, kind), FR.frame(size, 22, kind)
+                seen = {"x": 0.0, "w": 0.0}
+                with torch.no_grad():
+                    install(None, None, seen)
+                    st0 = R.source_pass(sd, hsd, src, ocfg)
+                    img0 = R.driver_pass(sd, hsd, st0, drv, ocfg)
+                    tlv0 = st0["target_latent_volume"]
+                    print(f"{size}^2 {kind:6s} largest |activation| into a source conv {seen['x']:.2f}, |weight| {seen['w']:.3f}",
+                          flush=True)
+                    st_fast = None
+                    for row, (src_fmt, dec_fmt) in SOURCE_FORMATS.items():
+                        install(src_fmt, None)
+                        if src_fmt is None:
+                            st = st0
+                        else:
+                            st = st_fast = st_fast or R.source_pass(sd, hsd, src, ocfg)
+                        install(None, dec_fmt)
+                        img = R.driver_pass(sd, hsd, st, drv, ocfg)
+                        install(None, None)
+                        err = (img - img0).abs()
+                        mse = (err ** 2).mean().item()
+                        psnr = 10 * math.log10(1.0 / mse) if mse > 0 else float("inf")
+                        u8, u80 = to_u8(img).int(), to_u8(img0).int()
+                        changed = (u8 != u80).float().mean().item()
+                        levels = (u8 - u80).abs().max().item()
+                        e_tlv = (st["target_latent_volume"] - tlv0).abs().max().item()
+                        print(f"{size}^2 {kind:6s} {row:36s} image max-abs {err.max().item():.1e} mean-abs {err.mean().item():.1e}  "
+                              f"PSNR {psnr:5.1f} dB  uint8 pixels moved {100 * changed:.2f} % (at most {levels} level)  "
+                              f"target_latent_volume max-abs {e_tlv:.1e} (of max {tlv0.abs().max().item():.2f})", flush=True)
+    finally:
+        F.conv2d, F.conv3d = conv2d, conv3d
+        for name, fn in nets.items():
+            setattr(R, name, fn)
+
+
 def main():
+    if "--source" in sys.argv:
+        kinds = [sys.argv[sys.argv.index("--frames") + 1]] if "--frames" in sys.argv else ["smooth", "noise"]
+        sizes = [int(a) for a in sys.argv[1:] if a.isdigit()] or [256, 512]
+        source_main(sizes, kinds)
+        return
     if "--stage2" in sys.argv:
         kinds = [sys.argv[sys.argv.index("--frames") + 1]] if "--frames" in sys.argv else ["smooth", "noise"]
         sizes = [int(a) for a in sys.argv[1:] if a.isdigit()] or [512, 1024]

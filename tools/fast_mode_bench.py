@@ -3,6 +3,7 @@
 
     python tools/fast_mode_bench.py [--steps K] [--warmup W] [--rounds R]
     python tools/fast_mode_bench.py --stage2 [--steps K] [--warmup W] [--rounds R]     (stage 2: see main_stage2)
+    python tools/fast_mode_bench.py --source [--steps K] [--warmup W] [--rounds R]     (the source pass: see main_source)
 
 Per mode, with bench.py's definitions (driver frame @512^2, shipped model, synthetic seed-0 weights, cached source identity):
   fps          device-resident driver frames/s, four captured frames in flight (infer.DriverPipeline depth 4), CUDA events
@@ -246,16 +247,127 @@ def main_stage2(args):
     print(json.dumps(line))
 
 
+class _Timed:
+    """a network of Model whose calls record a CUDA event before and after (on the current stream)"""
+
+    def __init__(self, net, events):
+        self.net, self.events = net, events
+
+    def __call__(self, *a, **k):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        out = self.net(*a, **k)
+        e1.record()
+        self.events.append((e0, e1))
+        return out
+
+
+def source_pass_times(model, src, reps):
+    """per source pass (eager, as the wrapper runs it), ms: total and the split LocalEncoder / VolumeSource + the two warps
+    (from the start of VolumeSource to the start of Unet3D) / Unet3D / rest; the median of `reps` passes"""
+    ev = {k: [] for k in ("le", "vs", "unet")}
+    nets = {"le": "local_encoder_nw", "vs": "volume_source_nw", "unet": "volume_process_nw"}
+    orig = {k: getattr(model, n) for k, n in nets.items()}
+    for k, n in nets.items():
+        setattr(model, n, _Timed(orig[k], ev[k]))
+    tot = []
+    try:
+        for _ in range(reps):
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            model.source_pass(src)
+            e1.record()
+            tot.append((e0, e1))
+        torch.cuda.synchronize()
+    finally:
+        for k, n in nets.items():
+            setattr(model, n, orig[k])
+    rows = []
+    for i in range(reps):
+        t = tot[i][0].elapsed_time(tot[i][1])
+        le = ev["le"][i][0].elapsed_time(ev["le"][i][1])
+        vs = ev["vs"][i][0].elapsed_time(ev["unet"][i][0])
+        un = ev["unet"][i][0].elapsed_time(ev["unet"][i][1])
+        rows.append(dict(source_pass_ms=t, local_encoder_ms=le, volume_source_and_warps_ms=vs, unet3d_ms=un, rest_ms=t - le - vs - un))
+    return {k: statistics.median(r[k] for r in rows) for k in rows[0]}
+
+
+def photo_to_photo_ms(wrapper, src, drv, reps):
+    """wall time of wrapper.forward(source, driver): one source pass and one driver frame, the PIL image back on the host"""
+    out = []
+    for _ in range(reps):
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        wrapper.forward(src, drv, crop=False, mix=True, mix_old=False)
+        torch.cuda.synchronize()
+        out.append((time.perf_counter() - t0) * 1000.0)
+    return statistics.median(out)
+
+
+def main_source(args):
+    """The source pass (notebooks/infer.py:374-507) exact vs source_precision="fast" @512^2 (bench.py's size, shipped model,
+    synthetic seed-0 weights, bench.frame(512, 0) as the source), the modes alternated over the rounds: the source pass's
+    device time per pass split by network (CUDA events, median of --steps passes after --warmup), and photo-to-photo latency,
+    InferenceWrapper.forward(source, driver) wall time including the PIL conversion (median of --steps // 4 calls)."""
+    import numpy as np
+
+    from emoportraits_b200.checkpoint import synthetic_head_pose_state_dict, synthetic_state_dict
+    from emoportraits_b200.config import shipped_config
+    from emoportraits_b200.infer import InferenceWrapper
+
+    cfg = shipped_config(bench.SIZE)
+    sd, hsd = synthetic_state_dict(cfg, 0), synthetic_head_pose_state_dict(0)
+    wrappers = {m: InferenceWrapper("bench", args_path=ROOT / "tests" / "golden" / f"args_{bench.SIZE}.txt", state_dict=sd,
+                                    head_pose_state_dict=hsd, print_params=False, source_precision=m) for m in ("exact", "fast")}
+    src = bench.frame(bench.SIZE, 0).cuda()
+    drv = bench.frame(bench.SIZE, 1000).cuda()
+    K, W = args.steps, max(args.warmup, 3)
+    runs = {m: [] for m in wrappers}
+    for _ in range(args.rounds):
+        for m, w in wrappers.items():
+            source_pass_times(w.model, src, W)
+            photo_to_photo_ms(w, src, drv, 2)
+            sampler = bench.ClockSampler(torch.cuda.current_device())
+            sampler.start()
+            r = source_pass_times(w.model, src, K)
+            r["photo_to_photo_ms"] = photo_to_photo_ms(w, src, drv, max(K // 4, 3))
+            r["clocks"] = sampler.stop()
+            runs[m].append(r)
+    res = {}
+    keys = ("source_pass_ms", "local_encoder_ms", "volume_source_and_warps_ms", "unet3d_ms", "rest_ms", "photo_to_photo_ms")
+    for m, rs in runs.items():
+        res[m] = {k: statistics.median(r[k] for r in rs) for k in keys}
+        res[m].update(source_pass_ms_runs=[r["source_pass_ms"] for r in rs], photo_to_photo_ms_runs=[r["photo_to_photo_ms"] for r in rs],
+                      clocks=[r["clocks"] for r in rs])
+    pil, img = {}, {}
+    for m, w in wrappers.items():
+        pil[m], img[m] = w.forward(src, drv, crop=False, mix=True, mix_old=False)
+    d = (img["fast"] - img["exact"]).abs()
+    u8 = {m: torch.from_numpy(np.asarray(pil[m][0])).int() for m in pil}
+    line = {"metric": "source pass with source_precision=fast (local encoder, volume blocks, 3-D U-Net on one fp16 operand "
+                      "plane; stem on the tensor cores) vs exact @512^2: source pass ms, photo-to-photo ms",
+            **_card(), "steps": K, "warmup": W, "rounds": args.rounds, "exact": res["exact"], "fast": res["fast"],
+            "speedup": {k: res["exact"][k] / res["fast"][k] for k in keys},
+            "image_vs_exact": {"max_abs": d.max().item(), "mean_abs": d.mean().item(),
+                               "uint8_moved": (u8["fast"] != u8["exact"]).float().mean().item(),
+                               "uint8_max_levels": (u8["fast"] - u8["exact"]).abs().max().item()}}
+    print(json.dumps(line))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=200)
     ap.add_argument("--warmup", type=int, default=10)
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--stage2", action="store_true", help="the stage-2 arm (main_stage2) instead of the stage-1 decoder's")
+    ap.add_argument("--source", action="store_true", help="the source-pass arm (main_source): source_precision exact vs fast")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "tools/fast_mode_bench.py measures on the GPU"
     if args.stage2:
         main_stage2(args)
+        return
+    if args.source:
+        main_source(args)
         return
     from emoportraits_b200.checkpoint import synthetic_head_pose_state_dict, synthetic_state_dict
     from emoportraits_b200.config import shipped_config
