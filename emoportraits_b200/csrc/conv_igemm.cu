@@ -53,8 +53,9 @@ struct ConvKParams {
   int ksplit;   // split-K factor: work item = (tile, K part); part `k` writes its partial sums to ws + k * ws_part_elems
   float* ws;    // split-K fp32 workspace [ksplit][N][Dout][Hout][Wout][Cout] (no initial state needed)
   long long ws_part_elems;
-  int dbg;    // EMO_CONV_DEBUG builds only (tools/conv_bound_probe.py): 1 skip TMA loads, 2 skip MMAs.  Results are garbage;
-              // only the timing is of interest.
+  int dbg;    // EMO_CONV_DEBUG builds only (tools/conv_bound_probe.py): 1 skip TMA loads, 2 skip MMAs, 4 skip the residual /
+              // post-add loads, 8 skip the output stores, 16 skip the statistics.  Results are garbage; only the timing is of
+              // interest.  256 phase stamps, 512 phase clocks (tools/conv_timeline.py).
   const float* bias;
   const float* residual;
   int res_shift;
@@ -186,8 +187,19 @@ __device__ __forceinline__ unsigned long long emo_gtime() {
   return t;
 }
 #define EMO_STAMP(k, cond) do { if ((p.dbg & 256) && (cond) && blockIdx.x < 160) g_conv_stamps[blockIdx.x * 16 + (k)] = emo_gtime(); } while (0)
+// Per-CTA phase clocks (EMO_CONV_DBG bit 512, tools/conv_timeline.py --phases): consumer thread 0 adds the SM clock cycles
+// since its previous mark to slot k, over ALL tiles of the launch (the host zeroes them): 0 waiting for operands, 1 issuing
+// the main loop and promoting its chunks, 2 final-phase loads (waited for), 3 activation and stores, 4 statistics and
+// barriers, 5 tile set-up (prefetch, bias); slot 7 counts the tiles.
+__device__ unsigned long long g_conv_phase[160 * 8];
+#define EMO_PHASE(k) do { if ((p.dbg & 512) && et == 0 && blockIdx.x < 160) { const long long t_ = clock64(); \
+    atomicAdd(&g_conv_phase[blockIdx.x * 8 + (k)], (unsigned long long)(t_ - ph_t)); ph_t = t_; } } while (0)
+// EMO_CONV_DBG bits that switch parts of the final phase off: 4 residual / post-add loads, 8 output stores, 16 statistics
+#define EMO_DBG(bits) ((p.dbg & (bits)) != 0)
 #else
 #define EMO_STAMP(k, cond) do { } while (0)
+#define EMO_PHASE(k) do { } while (0)
+#define EMO_DBG(bits) false
 #endif
 
 struct TMaps {
@@ -470,6 +482,9 @@ conv_igemm_kernel(const __grid_constant__ TMaps tm, const __grid_constant__ Conv
 
   int stage = 0, sa = 0, sb = 0;
   uint32_t phase = 0, pha = 0, phb = 0;
+#ifdef EMO_CONV_DEBUG
+  long long ph_t = clock64();
+#endif
   for (int item = tile_first; item < total_tiles; item += tile_step) {
     const int tile = item / ksplit, part = item - tile * ksplit;
     const int nks = (int)((long long)ksteps * (part + 1) / ksplit) - (int)((long long)ksteps * part / ksplit);
@@ -534,6 +549,7 @@ conv_igemm_kernel(const __grid_constant__ TMaps tm, const __grid_constant__ Conv
 #pragma unroll
       for (int j = 0; j < kMaxBN / 2; ++j) acc[j] = 0.f;
     }
+    EMO_PHASE(5);
 
     uint64_t* pend_b = nullptr;
     uint64_t* pend_a = nullptr;
@@ -544,12 +560,16 @@ conv_igemm_kernel(const __grid_constant__ TMaps tm, const __grid_constant__ Conv
       const uint32_t row_shift = (uint32_t)p.tw * KC * 2;  // one image row of the halo tile: a whole number of swizzle atoms
       int ks = 0;
       for (int gi = 0; gi < ngroups; ++gi) {
+        EMO_PHASE(1);
         mbar_wait(&afull_bar[sa], pha);
+        EMO_PHASE(0);
         EMO_STAMP(4, et == 0 && item == tile_first && gi == 0);
         for (int b = 0; b < p.kh; ++b, ++ks) {
           const bool chunk_first = (ks % F) == 0;
           const bool chunk_last = ((ks + 1) % F) == 0 || ks == nks - 1;
+          EMO_PHASE(1);
           mbar_wait(&full_bar[sb], phb);
+          EMO_PHASE(0);
           issue_kstep(n_tile, smem_u32(smem + (size_t)sa * a_halo_bytes) + (uint32_t)b * row_shift + wg_off, a_halo_plane,
                       smem_u32(b_ring + (size_t)sb * b_tile_bytes), chunk_first);
           // the halo tile is released with the last of its kh tap rows
@@ -562,7 +582,9 @@ conv_igemm_kernel(const __grid_constant__ TMaps tm, const __grid_constant__ Conv
       for (int ks = 0; ks < nks; ++ks) {
         const bool chunk_first = (ks % F) == 0;
         const bool chunk_last = ((ks + 1) % F) == 0 || ks == nks - 1;
+        EMO_PHASE(1);
         mbar_wait(&full_bar[stage], phase);
+        EMO_PHASE(0);
         EMO_STAMP(4, et == 0 && item == tile_first && ks == 0);
         const uint32_t st = smem_u32(smem + (size_t)stage * stage_bytes);
         issue_kstep(n_tile, st + wg_off, a_bytes, st + NP * a_bytes, chunk_first);
@@ -577,6 +599,10 @@ conv_igemm_kernel(const __grid_constant__ TMaps tm, const __grid_constant__ Conv
 #pragma unroll
       for (int j = 0; j < kMaxBN / 2; ++j) acc[j] *= p.out_scale;
     }
+    EMO_PHASE(1);
+#ifdef EMO_CONV_DEBUG
+    if ((p.dbg & 512) && et == 0 && blockIdx.x < 160) atomicAdd(&g_conv_phase[blockIdx.x * 8 + 7], 1ull);
+#endif
 
     // ---- final phase: this thread's two rows ----
     if (ksplit > 1) {
@@ -599,70 +625,103 @@ conv_igemm_kernel(const __grid_constant__ TMaps tm, const __grid_constant__ Conv
           }
         }
       }
+      EMO_PHASE(3);
       continue;
     }
     const long long sp = (long long)p.Dout * oHt * oWt;
-    const bool pairs = (p.Cout & 1) == 0;  // c even, Cout even: both columns of a pair exist, 8-byte aligned
+    // The final phase is unrolled over the 8-column blocks and both rows, so its code is long.  It is instantiated once per
+    // activation, with the odd-channel scalar path in an instantiation of its own: a tile then runs straight-line code that
+    // holds only what it executes.  A run-time activation switch and the scalar path inside every block would scatter the
+    // executed instructions over far more code than the instruction caches hold, fetched anew by every tile (DESIGN.md
+    // section 7).
+    auto final_rows = [&](auto pairs_c, auto act_c) {
+      constexpr bool pairs = decltype(pairs_c)::value;  // c even, Cout even: both columns of a pair exist, 8-byte aligned
+      constexpr int act_k = decltype(act_c)::value;
+      const int act = act_k >= 0 ? act_k : p.act;  // -1: the activation is read at run time (the scalar path)
 #pragma unroll
-    for (int rr = 0; rr < 2; ++rr) {
-      bool valid;
-      long long pix, rpix, spi;
-      locate(rr, valid, pix, rpix, spi);
-      // the row's residual / post-add values are loaded together before any store (a load may not move over a store that
-      // may alias it, so loads interleaved with the stores would each wait out a full memory latency); they are kept in the
-      // chunk registers, which are free until the next tile's main loop
+      for (int rr = 0; rr < 2; ++rr) {
+        bool valid;
+        long long pix, rpix, spi;
+        locate(rr, valid, pix, rpix, spi);
+        // the row's residual / post-add values are loaded together before any store (a load may not move over a store that
+        // may alias it, so loads interleaved with the stores would each wait out a full memory latency); they are kept in the
+        // chunk registers, which are free until the next tile's main loop
 #pragma unroll
-      for (int j = 0; j < kMaxBN / 8; ++j) {
-        const int c = n0 + 8 * j + cq;
-        float2 r2 = make_float2(0.f, 0.f), p2 = make_float2(0.f, 0.f);
-        if (8 * j < BN && pairs && valid && c < p.Cout) {
-          if (p.residual) r2 = __ldg((const float2*)(p.residual + rpix * p.Cout + c));
-          if (p.post_add) p2 = __ldg((const float2*)(p.post_add + spi * p.Cout + c));
+        for (int j = 0; j < kMaxBN / 8; ++j) {
+          const int c = n0 + 8 * j + cq;
+          float2 r2 = make_float2(0.f, 0.f), p2 = make_float2(0.f, 0.f);
+          if (8 * j < BN && pairs && valid && c < p.Cout && !EMO_DBG(4)) {
+            if (p.residual) r2 = __ldg((const float2*)(p.residual + rpix * p.Cout + c));
+            if (p.post_add) p2 = __ldg((const float2*)(p.post_add + spi * p.Cout + c));
+          }
+          cf[2 * j] = r2.x; cf[2 * j + 1] = r2.y; cf[kMaxBN / 4 + 2 * j] = p2.x; cf[kMaxBN / 4 + 2 * j + 1] = p2.y;
         }
-        cf[2 * j] = r2.x; cf[2 * j + 1] = r2.y; cf[kMaxBN / 4 + 2 * j] = p2.x; cf[kMaxBN / 4 + 2 * j + 1] = p2.y;
-      }
+#ifdef EMO_CONV_DEBUG
+        if (p.dbg & 512) {
+          // phase clocks: wait for the loads here, so that their latency is counted as load time
+          float s = 0.f;
 #pragma unroll
-      for (int j = 0; j < kMaxBN / 8; ++j) {
-        if (8 * j >= BN) continue;
-        const int c = n0 + 8 * j + cq;
-        float v0 = acc[4 * j + 2 * rr], v1 = acc[4 * j + 2 * rr + 1];
-        if (valid && c < p.Cout) {
-          if (pairs) {
-            v0 = act_apply(v0 + cf[2 * j], p.act) + cf[kMaxBN / 4 + 2 * j];
-            v1 = act_apply(v1 + cf[2 * j + 1], p.act) + cf[kMaxBN / 4 + 2 * j + 1];
-            if (!p.out_nchw) {
-              *(float2*)(p.out + pix * p.Cout + c) = make_float2(v0, v1);
+          for (int j = 0; j < kMaxBN / 2; ++j) s += cf[j];
+          if (s == 1.2345e-38f) g_conv_phase[0] = 0;
+        }
+#endif
+        EMO_PHASE(2);
+#pragma unroll
+        for (int j = 0; j < kMaxBN / 8; ++j) {
+          if (8 * j >= BN) continue;
+          const int c = n0 + 8 * j + cq;
+          float v0 = acc[4 * j + 2 * rr], v1 = acc[4 * j + 2 * rr + 1];
+          if (valid && c < p.Cout && !EMO_DBG(8)) {
+            if constexpr (pairs) {
+              // __fadd_rn: the post-add stays a separate rounding (never contracted into the activation's last multiply)
+              v0 = __fadd_rn(act_apply(v0 + cf[2 * j], act), cf[kMaxBN / 4 + 2 * j]);
+              v1 = __fadd_rn(act_apply(v1 + cf[2 * j + 1], act), cf[kMaxBN / 4 + 2 * j + 1]);
+              if (!p.out_nchw) {
+                *(float2*)(p.out + pix * p.Cout + c) = make_float2(v0, v1);
+              } else {
+                p.out[((long long)n * p.Cout + c) * sp + spi] = v0;
+                p.out[((long long)n * p.Cout + c + 1) * sp + spi] = v1;
+              }
             } else {
-              p.out[((long long)n * p.Cout + c) * sp + spi] = v0;
-              p.out[((long long)n * p.Cout + c + 1) * sp + spi] = v1;
+              // odd channel count (e.g. Cout = 3): scalar path
+#pragma unroll
+              for (int q = 0; q < 2; ++q) {
+                const int cc = c + q;
+                float x = q ? v1 : v0;
+                if (cc < p.Cout) {
+                  if (p.residual) x += __ldg(p.residual + rpix * p.Cout + cc);
+                  x = act_apply(x, act);
+                  if (p.post_add) x += __ldg(p.post_add + spi * p.Cout + cc);
+                  if (!p.out_nchw) p.out[pix * p.Cout + cc] = x;
+                  else p.out[((long long)n * p.Cout + cc) * sp + spi] = x;
+                } else {
+                  x = 0.f;
+                }
+                if (q) v1 = x; else v0 = x;
+              }
             }
           } else {
-            // odd channel count (e.g. Cout = 3): scalar path
-#pragma unroll
-            for (int q = 0; q < 2; ++q) {
-              const int cc = c + q;
-              float x = q ? v1 : v0;
-              if (cc < p.Cout) {
-                if (p.residual) x += __ldg(p.residual + rpix * p.Cout + cc);
-                x = act_apply(x, p.act);
-                if (p.post_add) x += __ldg(p.post_add + spi * p.Cout + cc);
-                if (!p.out_nchw) p.out[pix * p.Cout + cc] = x;
-                else p.out[((long long)n * p.Cout + cc) * sp + spi] = x;
-              } else {
-                x = 0.f;
-              }
-              if (q) v1 = x; else v0 = x;
-            }
+            v0 = 0.f; v1 = 0.f;  // pixels / channels outside the tensor: no part of the statistics
           }
-        } else {
-          v0 = 0.f; v1 = 0.f;  // pixels / channels outside the tensor: no part of the statistics
+          acc[4 * j + 2 * rr] = v0; acc[4 * j + 2 * rr + 1] = v1;
         }
-        acc[4 * j + 2 * rr] = v0; acc[4 * j + 2 * rr + 1] = v1;
+        EMO_PHASE(3);
+      }
+    };
+    using std::integral_constant;
+    if ((p.Cout & 1) != 0) {
+      final_rows(std::false_type{}, integral_constant<int, -1>{});
+    } else {
+      switch (p.act) {
+        case EMO_ACT_RELU: final_rows(std::true_type{}, integral_constant<int, EMO_ACT_RELU>{}); break;
+        case EMO_ACT_SIGMOID: final_rows(std::true_type{}, integral_constant<int, EMO_ACT_SIGMOID>{}); break;
+        case EMO_ACT_TANH: final_rows(std::true_type{}, integral_constant<int, EMO_ACT_TANH>{}); break;
+        default: final_rows(std::true_type{}, integral_constant<int, EMO_ACT_NONE>{}); break;
       }
     }
     EMO_STAMP(6, et == 0);
 
-    if (p.stats) {
+    if (p.stats && !EMO_DBG(16)) {
       // column sums of the warp's 16 rows: two rows in the thread, then a butterfly over the eight lanes sharing the columns
       float* cs = col_sum + warp * kMaxBN;
       float* cqs = col_sq + warp * kMaxBN;
@@ -688,6 +747,7 @@ conv_igemm_kernel(const __grid_constant__ TMaps tm, const __grid_constant__ Conv
       tile_group_stats(p, col_sum, col_sq, n, n0, BN, et, kConsumerWarps * 32);
       asm volatile("bar.sync 1, %0;" ::"n"(kConsumerWarps * 32) : "memory");  // the slots are rewritten by the next tile
     }
+    EMO_PHASE(4);
     EMO_STAMP(7, et == 0);
   }
   EMO_STAMP(8, et == 0);
@@ -1143,6 +1203,14 @@ using namespace emo;
 #ifdef EMO_CONV_DEBUG
 extern "C" int emo_debug_conv_stamps(unsigned long long* host160x16) {
   return cudaMemcpyFromSymbol(host160x16, g_conv_stamps, sizeof(unsigned long long) * 160 * 16) == cudaSuccess ? 0 : -2;
+}
+// the phase clocks (g_conv_phase) into host160x8; reset != 0: zero them instead
+extern "C" int emo_debug_conv_phases(unsigned long long* host160x8, int reset) {
+  if (reset) {
+    static const unsigned long long zeros[160 * 8] = {};
+    return cudaMemcpyToSymbol(g_conv_phase, zeros, sizeof(zeros)) == cudaSuccess ? 0 : -2;
+  }
+  return cudaMemcpyFromSymbol(host160x8, g_conv_phase, sizeof(unsigned long long) * 160 * 8) == cudaSuccess ? 0 : -2;
 }
 #endif
 
