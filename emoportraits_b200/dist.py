@@ -20,11 +20,30 @@ from .config import HotPathConfig
 
 
 def source_state_shapes(cfg: HotPathConfig):
+    """The identity: the fields of a source state that a driver frame reads (Model.driver_pass), besides
+    source_theta_dev, which is pred_source_theta[0] in every state (new_identity keeps it as that view).  The broadcast
+    sends these, and a captured driver graph (Model.make_driver_graph) holds its own copy of them."""
     return {
         "target_latent_volume": (1, cfg.D, cfg.S, cfg.S, cfg.C),
         "idt_embed": (1, cfg.idt_channels, cfg.embed_size, cfg.embed_size),
         "pred_source_theta": (1, 4, 4),
     }
+
+
+def new_identity(cfg: HotPathConfig, device) -> SimpleNamespace:
+    """zeroed fp32 identity buffers (source_state_shapes), with source_theta_dev the view pred_source_theta[0]"""
+    out = SimpleNamespace(**{k: torch.zeros(s, dtype=torch.float32, device=device) for k, s in source_state_shapes(cfg).items()})
+    out.source_theta_dev = out.pred_source_theta[0]
+    return out
+
+
+def check_identity(st, cfg: HotPathConfig) -> None:
+    """ValueError unless `st` carries every identity field as an fp32 tensor of the shape `cfg` gives it"""
+    for k, shp in source_state_shapes(cfg).items():
+        t = getattr(st, k, None)
+        if not isinstance(t, torch.Tensor) or tuple(t.shape) != shp or t.dtype != torch.float32:
+            got = (tuple(t.shape), t.dtype) if isinstance(t, torch.Tensor) else type(t).__name__
+            raise ValueError(f"not an identity of this model: {k} must be an fp32 tensor of shape {shp}, got {got}")
 
 
 def broadcast_source_state(st, cfg: HotPathConfig, device, src: int = 0, group=None):
@@ -41,13 +60,12 @@ def broadcast_source_state(st, cfg: HotPathConfig, device, src: int = 0, group=N
             flat[off:off + t.numel()].copy_(t)
             off += t.numel()
     dist.broadcast(flat, src=src, group=group)
-    out = SimpleNamespace()
+    out = new_identity(cfg, device)
     off = 0
     for k, shp in shapes.items():
         n = int(torch.tensor(shp).prod())
-        setattr(out, k, flat[off:off + n].view(shp).clone().contiguous())
+        getattr(out, k).copy_(flat[off:off + n].view(shp))
         off += n
-    out.source_theta_dev = out.pred_source_theta[0].contiguous()
     return out
 
 

@@ -22,6 +22,7 @@ import torch
 
 from . import nets, ops
 from .config import HotPathConfig, hot_path_config, parse_args
+from .dist import check_identity, new_identity, source_state_shapes
 
 
 class Model:
@@ -186,6 +187,9 @@ class Model:
                           smooth_state: Optional[torch.Tensor] = None, smooth_momentum: float = 0.5):
         """Capture one driver frame (all ~240 kernel launches) into a CUDA graph: removes the Python/ctypes launch
         overhead from the per-frame loop.  Returns replay(drv (1,3,H,W) on device) -> img (1,3,H,W) (static buffer).
+        The graph reads its identity from buffers of its own (replay.identity, dist.new_identity), never from `st`:
+        `st` is loaded into them before the capture, and replay.load(other) switches the identity of later replays without
+        a new capture.
         `slot` selects the scratch set (ops.set_slot) the captured frame uses; graphs that may replay concurrently on
         different streams need different slots.  smooth_state (3,4): the captured frame also smooths its pose into this
         tensor in place (smooth_pose=True, infer.py:571-581; the state must already be seeded by one eager frame) - frames of
@@ -199,28 +203,51 @@ class Model:
     def _make_driver_graph(self, st, mix, target_theta, mix_old=False, smooth_state=None, smooth_momentum=0.5):
         s = self.cfg.image_size
         static_in = torch.zeros((1, 3, s, s), dtype=torch.float32, device=self.device)
+        identity = new_identity(self.cfg, self.device)
         kw = dict(mix=mix, target_theta=target_theta, mix_old=mix_old)
         if smooth_state is not None:
             kw.update(smooth_state=smooth_state, smooth_momentum=smooth_momentum, smooth_init=False)
             saved = smooth_state.clone()  # the warm-up and capture passes smooth a dummy frame into the state: put it back after
-        side = torch.cuda.Stream(device=self.device)
-        side.wait_stream(torch.cuda.current_stream(self.device))
-        with torch.cuda.stream(side):
-            for _ in range(2):
-                self.driver_pass(st, static_in, **kw)
-        torch.cuda.current_stream(self.device).wait_stream(side)
-        torch.cuda.synchronize(self.device)
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph):
-            out = self.driver_pass(st, static_in, **kw)
-            static_out = out[0]
-        if smooth_state is not None:
-            smooth_state.copy_(saved)
 
         def replay(drv: torch.Tensor) -> torch.Tensor:
             static_in.copy_(drv, non_blocking=True)
             graph.replay()
             return static_out
+
+        # load must not refer to replay: a reference cycle would leave the graph to the cyclic garbage collector, which may
+        # then destroy it in the middle of another graph's capture (and so invalidate that capture)
+        loaded = [None]
+
+        def load(state) -> None:
+            """Make `state` the identity of the following replays: copy its identity fields into the graph's buffers on the
+            current stream (nothing to do if it is loaded already).  The graph keeps a reference to the loaded state, and
+            its tensors are marked as in use by the current stream, so a caller may drop the state before the copy ran."""
+            if loaded[0] is state:
+                return
+            check_identity(state, self.cfg)
+            cur = torch.cuda.current_stream(self.device)
+            for k in source_state_shapes(self.cfg):
+                src = getattr(state, k)
+                getattr(identity, k).copy_(src, non_blocking=True)
+                if src.is_cuda:
+                    src.record_stream(cur)
+            loaded[0] = state
+
+        replay.load, replay.identity = load, identity
+        load(st)  # the warm-up and capture passes run on a real identity
+        side = torch.cuda.Stream(device=self.device)
+        side.wait_stream(torch.cuda.current_stream(self.device))
+        with torch.cuda.stream(side):
+            for _ in range(2):
+                self.driver_pass(identity, static_in, **kw)
+        torch.cuda.current_stream(self.device).wait_stream(side)
+        torch.cuda.synchronize(self.device)
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph):
+            out = self.driver_pass(identity, static_in, **kw)
+            static_out = out[0]
+        if smooth_state is not None:
+            smooth_state.copy_(saved)
 
         replay.graph = graph
         replay.static_in, replay.static_out, replay.static_state = static_in, static_out, out[3]
@@ -233,30 +260,50 @@ class DriverPipeline:
     tiny launches (head-pose and expression encoders at 4^2..56^2) that leaves most SMs idle; replaying the captured
     frames of consecutive inputs on alternating streams lets one frame's big decoder kernels fill those holes.
     Frame i's result is produced in order on stream i % depth; nothing is batched and every frame runs the same
-    kernels as the single-stream path."""
+    kernels as the single-stream path.
+
+    Each slot's graph reads the identity from buffers of its own (Model.make_driver_graph), so frames of different
+    identities may be in flight at once: submit(..., st=) names the source state a frame animates.  A slot whose loaded
+    identity differs copies the new one in (~25 MB at 512^2) on its stream before the frame; nothing is re-captured.
+    The slots use scratch sets of their own (scratch_slots), apart from the eager passes' set 0, so a source pass may run
+    on the current stream while frames are in flight."""
 
     def __init__(self, model: "Model", st, depth: int = 2, mix: bool = True, target_theta: bool = True, mix_old: bool = False):
         self.model, self.depth, self.n = model, depth, 0
-        self.st = st  # the captured graphs hold raw pointers into this state's tensors: keep it alive as long as they are
+        self.st = st  # the current identity: frames submitted without st= animate it
         self.slots = []
-        for k in range(depth):
+        for k in self.scratch_slots(depth):
             run = model.make_driver_graph(st, mix=mix, target_theta=target_theta, slot=k, mix_old=mix_old)
             self.slots.append(SimpleNamespace(run=run, stream=torch.cuda.Stream(device=model.device),
                                               done=torch.cuda.Event(), busy=False))
 
-    def submit(self, drv: torch.Tensor, host_out: Optional[torch.Tensor] = None, dev_out: Optional[torch.Tensor] = None):
+    @staticmethod
+    def scratch_slots(depth: int) -> list:
+        """the scratch set (ops.set_slot) of each pipeline slot: 1 .. depth.  Set 0 belongs to the eager passes
+        (Model.source_pass / driver_pass on the current stream), which may overlap frames in flight."""
+        return [k + 1 for k in range(depth)]
+
+    def submit(self, drv: torch.Tensor, host_out: Optional[torch.Tensor] = None, dev_out: Optional[torch.Tensor] = None,
+               st=None):
         """Queue one frame (device tensor, or pinned host tensor -> asynchronous H2D on the frame's stream).  If `host_out`
         (pinned) / `dev_out` is given the image is copied into it on the same stream.  Returns a ticket: ticket.done is an
         event recorded when this frame (and its copy-out) has finished (ticket.slot.done is the same event, i.e. always the
         slot's latest frame); slot.run.static_out is valid until the slot's next submit.  A slot's frames are ordered by
         its stream, so a caller may queue further frames on a busy slot — it only has to keep the host_out / dev_out
-        buffers of unfinished frames apart."""
+        buffers of unfinished frames apart.
+        st: the source state (Model.source_pass, dist.broadcast_source_state) to animate; it becomes the pipeline's
+        current identity.  None: the current identity.  The frame's stream waits for the current stream first, so a
+        state whose source pass was just queued there may be given at once, and the caller may drop it after this call."""
+        if st is not None:
+            check_identity(st, self.model.cfg)
+            self.st = st
         sl = self.slots[self.n % self.depth]
         self.n += 1
         if not drv.is_contiguous():
             drv = drv.contiguous()  # a strided host tensor would otherwise take torch's staged, synchronous copy path
         sl.stream.wait_stream(torch.cuda.current_stream(self.model.device))
         with torch.cuda.stream(sl.stream):
+            sl.run.load(self.st)
             sl.run.static_in.copy_(drv, non_blocking=True)
             sl.run.graph.replay()
             if host_out is not None:
@@ -351,9 +398,40 @@ class InferenceWrapper(torch.nn.Module):
             raise NotImplementedError("get_mask needs the external MODNet network: set wrapper.modnet = <module>")
         return modnet_get_mask(self.modnet, img.to(self.device))
 
+    @property
+    def identity(self):
+        """The current identity, as an opaque handle: the source state of the last source pass, or the handle assigned last.
+        Assigning a handle read earlier makes its identity current again with no source pass and no graph capture: the
+        cached source attributes (idt_embed, pred_source_theta, target_latent_volume, source_image, ...) return to it and
+        the next driver frames animate it.  Each handle kept keeps its identity resident on the device: about 3 x 25 MB at
+        512^2 (the source, warped and processed latent volumes)."""
+        return self._state
+
+    @identity.setter
+    def identity(self, st):
+        check_identity(st, self.cfg)
+        if not hasattr(st, "wrapper_inputs"):
+            raise ValueError("identity: assign a handle read from InferenceWrapper.identity (it carries the source image and "
+                             "mask of its source pass)")
+        self._use_identity(st)
+
+    def _use_identity(self, st):
+        self._state = st
+        for k, v in st.wrapper_inputs.items():   # source_image, source_img_mask, ... as the source pass's forward set them
+            setattr(self, k, v)
+        # cached attributes of the reference wrapper (infer.py:405-507)
+        self.idt_embed = st.idt_embed
+        self.pred_source_theta = st.pred_source_theta
+        self.pred_source_pose_embed = st.pred_source_pose_embed
+        self.source_latent_volume = st.source_latent_volume.permute(0, 4, 1, 2, 3)       # NCDHW views
+        self.source_xy_warp_resize = st.source_xy_warp_resize
+        self.target_latent_volume_1 = st.target_latent_volume_1.permute(0, 4, 1, 2, 3)
+        self.target_latent_volume = st.target_latent_volume.permute(0, 4, 1, 2, 3)
+
     def _driver_pipeline(self, mix, target_theta, mix_old):
+        """the captured four-in-flight pipeline of these pose options; it serves every identity (submit(..., st=))"""
         key = (bool(mix), bool(target_theta), bool(mix_old))
-        if self._pipeline is None or self._pipeline.st is not self._state or self._pipeline_key != key:
+        if self._pipeline is None or self._pipeline_key != key:
             self._pipeline, self._pipeline_key = DriverPipeline(self.model, self._state, depth=4, mix=mix,
                                                                 target_theta=target_theta, mix_old=mix_old), key
         return self._pipeline
@@ -373,7 +451,7 @@ class InferenceWrapper(torch.nn.Module):
         for i, f in enumerate(frames):
             t = self._prep(f)
             keep.append(t)  # read by the slot's stream later: must not return to the allocator (of the current stream) before
-            sl = pipe.submit(t, dev_out=img[i:i + 1]).slot
+            sl = pipe.submit(t, dev_out=img[i:i + 1], st=self._state).slot
             with torch.cuda.stream(sl.stream):
                 ops.image_to_u8(img[i:i + 1], out=u8[i:i + 1])  # clamp(0, 1) + ToPILImage (mul(255).byte()) on the device
                 host[i].copy_(u8[i], non_blocking=True)
@@ -462,16 +540,10 @@ class InferenceWrapper(torch.nn.Module):
             self.source_img = self.source_img_crop_m = src
             st = self.model.source_pass(src, mask=mask, c_source_latent_volume=c_source_latent_volume,
                                         c_target_latent_volume=c_target_latent_volume)
-            self._state = st
-            self._pipeline = None  # captured for the previous identity
-            # cached attributes of the reference wrapper (infer.py:405-507)
-            self.idt_embed = st.idt_embed
-            self.pred_source_theta = st.pred_source_theta
-            self.pred_source_pose_embed = st.pred_source_pose_embed
-            self.source_latent_volume = st.source_latent_volume.permute(0, 4, 1, 2, 3)       # NCDHW views
-            self.source_xy_warp_resize = st.source_xy_warp_resize
-            self.target_latent_volume_1 = st.target_latent_volume_1.permute(0, 4, 1, 2, 3)
-            self.target_latent_volume = st.target_latent_volume.permute(0, 4, 1, 2, 3)
+            st.wrapper_inputs = dict(source_image=self.source_image, source_image_crop=self.source_image_crop,
+                                     source_img_mask=self.source_img_mask, source_img=self.source_img,
+                                     source_img_crop_m=self.source_img_crop_m)
+            self._use_identity(st)  # the captured driver graphs load it on their next frame; nothing is re-captured
 
         if driver_image is None:
             return None
@@ -490,7 +562,7 @@ class InferenceWrapper(torch.nn.Module):
             self._driver_pipeline(mix, target_theta, mix_old)
             img = torch.empty_like(drv)
             for i in range(drv.shape[0]):
-                sl = self._pipeline.submit(drv[i:i + 1], dev_out=img[i:i + 1]).slot
+                sl = self._pipeline.submit(drv[i:i + 1], dev_out=img[i:i + 1], st=self._state).slot
             self._pipeline.drain()
             so = sl.run.static_state
             self.pred_target_theta = so.pred_target_theta.clone()
@@ -498,22 +570,23 @@ class InferenceWrapper(torch.nn.Module):
             self.target_pose_embed = so.target_pose_embed.clone()
         elif smooth_pose and custom_srt is None and custome_target_pose_embed is None:
             # pose smoothing is a recurrence over the frames (infer.py:571-581): the first frame seeds self.theta eagerly, every
-            # further frame replays a captured graph that smooths into the same tensor, one after the other on this stream
+            # further frame replays a captured graph that smooths into the same tensor, one after the other on this stream.
+            # A reset seeds the captured graph's own state tensor, and a new identity is loaded into it: neither re-captures
             imgs = []
             for i in range(drv.shape[0]):
+                g = self._smooth_graph
                 if self.theta is None:
-                    self.theta = torch.zeros((3, 4), dtype=torch.float32, device=self.device)
+                    self.theta = g.theta if g is not None else torch.zeros((3, 4), dtype=torch.float32, device=self.device)
                     im, _, _, so = self.model.driver_pass(self._state, drv[i:i + 1].contiguous(), mix=mix, target_theta=target_theta,
                                                           mix_old=mix_old, smooth_state=self.theta, smooth_momentum=self.pose_momentum,
                                                           smooth_init=True)
-                    self._smooth_graph = None
                 else:
                     key = (bool(mix), bool(target_theta), bool(mix_old), float(self.pose_momentum))
-                    g = self._smooth_graph
-                    if g is None or g.st is not self._state or g.theta is not self.theta or g.key != key:
+                    if g is None or g.theta is not self.theta or g.key != key:
                         run = self.model.make_driver_graph(self._state, mix=mix, target_theta=target_theta, mix_old=mix_old,
                                                            smooth_state=self.theta, smooth_momentum=self.pose_momentum)
-                        g = self._smooth_graph = SimpleNamespace(run=run, st=self._state, theta=self.theta, key=key)
+                        g = self._smooth_graph = SimpleNamespace(run=run, theta=self.theta, key=key)
+                    g.run.load(self._state)
                     im, so = g.run(drv[i:i + 1]).clone(), g.run.static_state
                 imgs.append(im)
             img = imgs[0] if len(imgs) == 1 else torch.cat(imgs)
