@@ -30,9 +30,11 @@ def source_state_shapes(cfg: HotPathConfig):
     }
 
 
-def new_identity(cfg: HotPathConfig, device) -> SimpleNamespace:
-    """zeroed fp32 identity buffers (source_state_shapes), with source_theta_dev the view pred_source_theta[0]"""
-    out = SimpleNamespace(**{k: torch.zeros(s, dtype=torch.float32, device=device) for k, s in source_state_shapes(cfg).items()})
+def new_identity(cfg: HotPathConfig, device, fields=None) -> SimpleNamespace:
+    """zeroed fp32 identity buffers (source_state_shapes, or only the names in `fields`, which must include
+    pred_source_theta), with source_theta_dev the view pred_source_theta[0]"""
+    shapes = source_state_shapes(cfg)
+    out = SimpleNamespace(**{k: torch.zeros(shapes[k], dtype=torch.float32, device=device) for k in (fields or shapes)})
     out.source_theta_dev = out.pred_source_theta[0]
     return out
 

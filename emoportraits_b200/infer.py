@@ -14,6 +14,7 @@ stubbed reference oracle uses too) and `modnet_mask=True` raises.
 from __future__ import annotations
 
 import pathlib
+from collections import OrderedDict
 from types import SimpleNamespace
 from typing import Optional
 
@@ -144,28 +145,40 @@ class Model:
     def driver_pass(self, st, drv: torch.Tensor, mix: bool = True, target_theta: bool = True, taps: Optional[dict] = None,
                     want_logits: bool = False, pose_override=None, mix_old: bool = False,
                     custom_srt: Optional[torch.Tensor] = None, custom_pose_embed: Optional[torch.Tensor] = None,
-                    smooth_state: Optional[torch.Tensor] = None, smooth_momentum: float = 0.5, smooth_init: bool = False):
+                    smooth_state: Optional[torch.Tensor] = None, smooth_momentum: float = 0.5, smooth_init: bool = False,
+                    encode_only: bool = False):
         """drv (1,3,H,W) fp32 on device -> (img (1,3,H,W), feat_2d, img_feat, state).
         mix / mix_old: get_mixing_theta (infer.py:569-570, 686-736).  custom_srt (1,9) = the caller's
         custome_target_theta_embed (scale, rotation, translation) replacing the regressed pose (:566-567).
         custom_pose_embed (1,128) replaces the expression embedding (:602-603).  smooth_state (3,4) on device: the
-        wrapper's self.theta, smoothed in place with smooth_momentum (smooth_pose=True, :571-581)."""
+        wrapper's self.theta, smoothed in place with smooth_momentum (smooth_pose=True, :571-581).
+        drv=None (both custom_srt and custom_pose_embed given): an image-free frame, without the head-pose regressor and the
+        expression encoder; state.srt is then custom_srt.  encode_only: stop after the expression encoder and return
+        (None, None, None, state): the frame's regressed pose state.srt and its embedding state.target_pose_embed, whose 2-D
+        alignment comes from the mixed pose (so it depends on mix / mix_old and, with mix, on st's source pose)."""
         cfg = self.cfg
-        drv = drv.contiguous().float()
+        if drv is None and (custom_srt is None or custom_pose_embed is None or encode_only or taps is not None):
+            raise ValueError("driver_pass: a frame without a driver image needs custom_srt and custom_pose_embed")
+        if drv is not None:
+            drv = drv.contiguous().float()
         ops.begin_pass(self.device)
-        srt = self.head_pose_regressor(drv)
+        srt = None if drv is None else self.head_pose_regressor(drv)
         srt_used = srt if custom_srt is None else custom_srt.to(self.device).float().reshape(1, 9).contiguous()
+        if srt is None:
+            srt = srt_used     # an image-free frame reports the supplied pose
         theta, warp, align = ops.pose_theta(srt_used, source_theta=st.source_theta_dev if mix else None, mix=mix,
                                             mix_old=mix_old, smooth_state=smooth_state, smooth_momentum=smooth_momentum,
                                             smooth_init=smooth_init)
         if pose_override is not None:
             theta, warp, align = [t.to(self.device).float().contiguous() for t in pose_override]
-        if not target_theta:
-            warp = st.pred_source_theta[:, :3].contiguous()
         if custom_pose_embed is not None and taps is None:
             pose_embed, aligned = None, None      # the expression encoder's output would be discarded (infer.py:602-603)
         else:
             pose_embed, aligned = self.expression_embedder_nw(drv, align, want_aligned=taps is not None)
+        if encode_only:
+            return None, None, None, SimpleNamespace(pred_target_theta=theta, target_pose_embed=pose_embed, srt=srt)
+        if not target_theta:
+            warp = st.pred_source_theta[:, :3].contiguous()
         if custom_pose_embed is not None:
             pose_embed = custom_pose_embed.to(self.device).float().reshape(1, -1).contiguous()
         E = self.predict_embed(pose_embed, st.idt_embed)
@@ -183,8 +196,19 @@ class Model:
         return img, deep_f, img_f, st_out
 
 
+    @staticmethod
+    def check_inputs(image: bool, theta_embed: bool, pose_embed: bool, encode: bool) -> None:
+        """ValueError unless the inputs a captured frame reads are a valid set: a driver image, and / or the caller's
+        pose (theta_embed) and expression embedding (pose_embed); an image-free frame takes both, an encoding frame
+        (encode: the pose and the embedding of its image, no rendering) only the image"""
+        if not image and not (theta_embed and pose_embed):
+            raise ValueError("a frame without a driver image needs both theta_embed and pose_embed")
+        if encode and not (image and not theta_embed and not pose_embed):
+            raise ValueError("an encoding frame reads a driver image and nothing else")
+
     def make_driver_graph(self, st, mix: bool = True, target_theta: bool = True, slot: int = 0, mix_old: bool = False,
-                          smooth_state: Optional[torch.Tensor] = None, smooth_momentum: float = 0.5):
+                          smooth_state: Optional[torch.Tensor] = None, smooth_momentum: float = 0.5, image: bool = True,
+                          theta_embed: bool = False, pose_embed: bool = False, encode: bool = False):
         """Capture one driver frame (all ~240 kernel launches) into a CUDA graph: removes the Python/ctypes launch
         overhead from the per-frame loop.  Returns replay(drv (1,3,H,W) on device) -> img (1,3,H,W) (static buffer).
         The graph reads its identity from buffers of its own (replay.identity, dist.new_identity), never from `st`:
@@ -193,18 +217,33 @@ class Model:
         `slot` selects the scratch set (ops.set_slot) the captured frame uses; graphs that may replay concurrently on
         different streams need different slots.  smooth_state (3,4): the captured frame also smooths its pose into this
         tensor in place (smooth_pose=True, infer.py:571-581; the state must already be seeded by one eager frame) - frames of
-        such a graph are a recurrence and must replay one after the other on one stream."""
+        such a graph are a recurrence and must replay one after the other on one stream.
+        The inputs the graph reads (check_inputs), each from a static buffer of its own that the caller fills before a
+        replay: image -> replay.static_in (1,3,H,W); theta_embed -> replay.static_theta (1,9), the caller's (scale,
+        rotation, translation) in place of the regressed pose; pose_embed -> replay.static_pose (1,E), the caller's
+        expression embedding (the expression encoder is then not captured).  Without an image the head-pose regressor is
+        not captured either.  encode: the graph stops after the expression encoder (driver_pass(encode_only=True)):
+        replay.static_state.srt / .target_pose_embed are the frame's pose and embedding, static_out is None, and its
+        identity buffers hold only the source pose, the one identity field the embedding depends on."""
+        self.check_inputs(image, theta_embed, pose_embed, encode)
         prev = ops.set_slot(slot)
         try:
-            return self._make_driver_graph(st, mix, target_theta, mix_old, smooth_state, smooth_momentum)
+            return self._make_driver_graph(st, mix, target_theta, mix_old, smooth_state, smooth_momentum, image, theta_embed,
+                                           pose_embed, encode)
         finally:
             ops.set_slot(prev)
 
-    def _make_driver_graph(self, st, mix, target_theta, mix_old=False, smooth_state=None, smooth_momentum=0.5):
-        s = self.cfg.image_size
-        static_in = torch.zeros((1, 3, s, s), dtype=torch.float32, device=self.device)
-        identity = new_identity(self.cfg, self.device)
-        kw = dict(mix=mix, target_theta=target_theta, mix_old=mix_old)
+    def _make_driver_graph(self, st, mix, target_theta, mix_old=False, smooth_state=None, smooth_momentum=0.5, image=True,
+                           theta_embed=False, pose_embed=False, encode=False):
+        s, dev = self.cfg.image_size, self.device
+        static_in = torch.zeros((1, 3, s, s), dtype=torch.float32, device=dev) if image else None
+        # the warm-up passes run on the unit pose (scale 1, no rotation or translation) and a zero embedding
+        static_theta = torch.tensor([[1.0, 1, 1, 0, 0, 0, 0, 0, 0]], device=dev) if theta_embed else None
+        static_pose = torch.zeros((1, self.cfg.expr_channels), dtype=torch.float32, device=dev) if pose_embed else None
+        fields = ("pred_source_theta",) if encode else tuple(source_state_shapes(self.cfg))
+        identity = new_identity(self.cfg, dev, fields)
+        kw = dict(mix=mix, target_theta=target_theta, mix_old=mix_old, custom_srt=static_theta, custom_pose_embed=static_pose,
+                  encode_only=encode)
         if smooth_state is not None:
             kw.update(smooth_state=smooth_state, smooth_momentum=smooth_momentum, smooth_init=False)
             saved = smooth_state.clone()  # the warm-up and capture passes smooth a dummy frame into the state: put it back after
@@ -226,7 +265,7 @@ class Model:
                 return
             check_identity(state, self.cfg)
             cur = torch.cuda.current_stream(self.device)
-            for k in source_state_shapes(self.cfg):
+            for k in fields:
                 src = getattr(state, k)
                 getattr(identity, k).copy_(src, non_blocking=True)
                 if src.is_cuda:
@@ -251,6 +290,7 @@ class Model:
 
         replay.graph = graph
         replay.static_in, replay.static_out, replay.static_state = static_in, static_out, out[3]
+        replay.static_theta, replay.static_pose = static_theta, static_pose
         return replay
 
 
@@ -266,14 +306,22 @@ class DriverPipeline:
     identities may be in flight at once: submit(..., st=) names the source state a frame animates.  A slot whose loaded
     identity differs copies the new one in (~25 MB at 512^2) on its stream before the frame; nothing is re-captured.
     The slots use scratch sets of their own (scratch_slots), apart from the eager passes' set 0, so a source pass may run
-    on the current stream while frames are in flight."""
+    on the current stream while frames are in flight.
 
-    def __init__(self, model: "Model", st, depth: int = 2, mix: bool = True, target_theta: bool = True, mix_old: bool = False):
+    image / theta_embed / pose_embed name the inputs every frame takes (Model.make_driver_graph): the driver image, and the
+    caller's pose (1,9) and expression embedding (1,E) for the frame.  encode: each frame stops after the expression
+    encoder; its pose and embedding are slot.run.static_state.srt / .target_pose_embed."""
+
+    def __init__(self, model: "Model", st, depth: int = 2, mix: bool = True, target_theta: bool = True, mix_old: bool = False,
+                 image: bool = True, theta_embed: bool = False, pose_embed: bool = False, encode: bool = False):
+        model.check_inputs(image, theta_embed, pose_embed, encode)
         self.model, self.depth, self.n = model, depth, 0
+        self.image, self.theta_embed, self.pose_embed, self.encode = image, theta_embed, pose_embed, encode
         self.st = st  # the current identity: frames submitted without st= animate it
         self.slots = []
         for k in self.scratch_slots(depth):
-            run = model.make_driver_graph(st, mix=mix, target_theta=target_theta, slot=k, mix_old=mix_old)
+            run = model.make_driver_graph(st, mix=mix, target_theta=target_theta, slot=k, mix_old=mix_old, image=image,
+                                          theta_embed=theta_embed, pose_embed=pose_embed, encode=encode)
             self.slots.append(SimpleNamespace(run=run, stream=torch.cuda.Stream(device=model.device),
                                               done=torch.cuda.Event(), busy=False))
 
@@ -283,8 +331,23 @@ class DriverPipeline:
         (Model.source_pass / driver_pass on the current stream), which may overlap frames in flight."""
         return [k + 1 for k in range(depth)]
 
-    def submit(self, drv: torch.Tensor, host_out: Optional[torch.Tensor] = None, dev_out: Optional[torch.Tensor] = None,
-               st=None):
+    def _check_submit(self, drv, theta_embed, pose_embed, outs) -> None:
+        """ValueError unless a frame's inputs are the ones the pipeline was captured for, of the right shapes"""
+        given = dict(image=drv is not None, theta_embed=theta_embed is not None, pose_embed=pose_embed is not None)
+        want = dict(image=self.image, theta_embed=self.theta_embed, pose_embed=self.pose_embed)
+        if given != want:
+            raise ValueError(f"this pipeline was captured for the inputs {sorted(k for k, v in want.items() if v)}, "
+                             f"got {sorted(k for k, v in given.items() if v)}")
+        shapes = dict(theta_embed=(theta_embed, (1, 9)), pose_embed=(pose_embed, (1, self.model.cfg.expr_channels)))
+        for name, (t, shp) in shapes.items():
+            if t is not None and (not isinstance(t, torch.Tensor) or tuple(t.shape) != shp):
+                got = tuple(t.shape) if isinstance(t, torch.Tensor) else type(t).__name__
+                raise ValueError(f"{name} must be a tensor of shape {shp}, got {got}")
+        if self.encode and any(o is not None for o in outs):
+            raise ValueError("an encoding pipeline renders no image: host_out / dev_out must be None")
+
+    def submit(self, drv: Optional[torch.Tensor], host_out: Optional[torch.Tensor] = None, dev_out: Optional[torch.Tensor] = None,
+               st=None, theta_embed: Optional[torch.Tensor] = None, pose_embed: Optional[torch.Tensor] = None):
         """Queue one frame (device tensor, or pinned host tensor -> asynchronous H2D on the frame's stream).  If `host_out`
         (pinned) / `dev_out` is given the image is copied into it on the same stream.  Returns a ticket: ticket.done is an
         event recorded when this frame (and its copy-out) has finished (ticket.slot.done is the same event, i.e. always the
@@ -293,18 +356,25 @@ class DriverPipeline:
         buffers of unfinished frames apart.
         st: the source state (Model.source_pass, dist.broadcast_source_state) to animate; it becomes the pipeline's
         current identity.  None: the current identity.  The frame's stream waits for the current stream first, so a
-        state whose source pass was just queued there may be given at once, and the caller may drop it after this call."""
+        state whose source pass was just queued there may be given at once, and the caller may drop it after this call.
+        theta_embed (1,9) / pose_embed (1,E): the frame's pose and expression embedding, for a pipeline captured to take
+        them; they are copied into the slot's buffers on its stream like the image.  drv is None for an image-free
+        pipeline.  Inputs other than the pipeline's, or of other shapes, raise ValueError before anything is queued."""
         if st is not None:
             check_identity(st, self.model.cfg)
+        self._check_submit(drv, theta_embed, pose_embed, (host_out, dev_out))
+        if st is not None:
             self.st = st
         sl = self.slots[self.n % self.depth]
         self.n += 1
-        if not drv.is_contiguous():
-            drv = drv.contiguous()  # a strided host tensor would otherwise take torch's staged, synchronous copy path
+        # a strided host tensor would otherwise take torch's staged, synchronous copy path
+        inputs = [(buf, t if t.is_contiguous() else t.contiguous()) for buf, t in
+                  ((sl.run.static_in, drv), (sl.run.static_theta, theta_embed), (sl.run.static_pose, pose_embed)) if t is not None]
         sl.stream.wait_stream(torch.cuda.current_stream(self.model.device))
-        with torch.cuda.stream(sl.stream):
+        with torch.cuda.stream(sl.stream), torch.no_grad():
             sl.run.load(self.st)
-            sl.run.static_in.copy_(drv, non_blocking=True)
+            for buf, t in inputs:
+                buf.copy_(t, non_blocking=True)
             sl.run.graph.replay()
             if host_out is not None:
                 host_out.copy_(sl.run.static_out, non_blocking=True)
@@ -383,7 +453,7 @@ class InferenceWrapper(torch.nn.Module):
         self.resize_warp = False
         self.use_seg = getattr(self.args, 'use_seg', True)
         self._state = None
-        self._pipeline = self._pipeline_key = None
+        self._pipelines = OrderedDict()   # captured DriverPipelines by options, least recently used first
         self._smooth_graph = None
         # external mask networks (separate checkouts in the reference: repos/face_par_off behind model.face_idt, infer.py:410;
         # repos/MODNet, infer.py:140-149): None until the caller plugs them in (masks.FaceParsing(None, net=...), any MODNet module)
@@ -428,30 +498,48 @@ class InferenceWrapper(torch.nn.Module):
         self.target_latent_volume_1 = st.target_latent_volume_1.permute(0, 4, 1, 2, 3)
         self.target_latent_volume = st.target_latent_volume.permute(0, 4, 1, 2, 3)
 
-    def _driver_pipeline(self, mix, target_theta, mix_old):
-        """the captured four-in-flight pipeline of these pose options; it serves every identity (submit(..., st=))"""
-        key = (bool(mix), bool(target_theta), bool(mix_old))
-        if self._pipeline is None or self._pipeline_key != key:
-            self._pipeline, self._pipeline_key = DriverPipeline(self.model, self._state, depth=4, mix=mix,
-                                                                target_theta=target_theta, mix_old=mix_old), key
-        return self._pipeline
+    # Captured pipelines a wrapper keeps, one per set of options (pose options, the inputs a frame takes, encoding or
+    # rendering); the least recently used is dropped for a new one.  Plain frames, encode(), animate() and forward with an
+    # embedding then alternate with no capture.
+    PIPELINES = 4
 
-    def _forward_list(self, frames, mix, target_theta, mix_old):
+    def _driver_pipeline(self, mix, target_theta, mix_old, **inputs):
+        """the captured four-in-flight pipeline of these options (DriverPipeline's image / theta_embed / pose_embed / encode);
+        it serves every identity (submit(..., st=))"""
+        key = (bool(mix), bool(target_theta), bool(mix_old), tuple(sorted(inputs.items())))
+        pipe = self._pipelines.pop(key, None)
+        if pipe is None:
+            pipe = DriverPipeline(self.model, self._state, depth=4, mix=mix, target_theta=target_theta, mix_old=mix_old, **inputs)
+        self._pipelines[key] = pipe
+        # the new pipeline's captures synchronized the device, so nothing of a dropped one is still running
+        while len(self._pipelines) > self.PIPELINES:
+            self._pipelines.popitem(last=False)
+        return pipe
+
+    def _forward_list(self, frames, mix, target_theta, mix_old, theta_embed=None, pose_embed=None):
         """A list of PIL / numpy driver frames: every frame is converted, uploaded and queued on its own (four captured frames in
         flight), its uint8 image is produced and copied back on the frame's stream, so the host-side conversions of frame i + 1
-        overlap the device work of frame i; the PIL images are wrapped as their copies land.  Same results as one call per frame."""
+        overlap the device work of frame i; the PIL images are wrapped as their copies land.  Same results as one call per frame.
+        theta_embed (1,9) / pose_embed (1,E) on the device: the caller's pose / embedding for every frame."""
+        pipe = self._driver_pipeline(mix, target_theta, mix_old, theta_embed=theta_embed is not None,
+                                     pose_embed=pose_embed is not None)
+        return self._render(pipe, len(frames), lambda i: dict(drv=self._prep(frames[i]), theta_embed=theta_embed,
+                                                              pose_embed=pose_embed))
+
+    def _render(self, pipe, n, inputs):
+        """n frames through `pipe`, frame i with the submit arguments inputs(i), returned as forward returns them; sets the
+        pred_target_* attributes from the last frame"""
         from PIL import Image
 
-        pipe = self._driver_pipeline(mix, target_theta, mix_old)
-        n, s = len(frames), self.cfg.image_size
+        s = self.cfg.image_size
         img = torch.empty((n, 3, s, s), dtype=torch.float32, device=self.device)
         u8 = torch.empty((n, s, s, 3), dtype=torch.uint8, device=self.device)
         host = torch.empty((n, s, s, 3), dtype=torch.uint8).pin_memory()
         keep, done = [], []
-        for i, f in enumerate(frames):
-            t = self._prep(f)
-            keep.append(t)  # read by the slot's stream later: must not return to the allocator (of the current stream) before
-            sl = pipe.submit(t, dev_out=img[i:i + 1], st=self._state).slot
+        for i in range(n):
+            kw = inputs(i)
+            keep.append(kw)  # read by the slot's stream later: must not return to the allocator (of the current stream) before
+            sl = pipe.submit(dev_out=img[i:i + 1], st=self._state, **kw).slot
             with torch.cuda.stream(sl.stream):
                 ops.image_to_u8(img[i:i + 1], out=u8[i:i + 1])  # clamp(0, 1) + ToPILImage (mul(255).byte()) on the device
                 host[i].copy_(u8[i], non_blocking=True)
@@ -470,6 +558,73 @@ class InferenceWrapper(torch.nn.Module):
         self.pred_target_srt = (so.srt[:, :3].clone(), so.srt[:, 3:6].clone(), so.srt[:, 6:9].clone())
         self.target_pose_embed = so.target_pose_embed.clone()
         return pred_target_img, img
+
+    def _frames(self, driver_images):
+        """(n, frame(i) -> (1,3,S,S) on the device): a list of PIL / numpy frames is converted frame by frame, as it is
+        queued; anything else (a tensor, one image) at once"""
+        if isinstance(driver_images, list) and driver_images and not isinstance(driver_images[0], torch.Tensor):
+            return len(driver_images), lambda i: self._prep(driver_images[i])
+        drv = self._prep(driver_images)
+        return drv.shape[0], lambda i: drv[i:i + 1]
+
+    @torch.no_grad()
+    def encode(self, driver_images, mix=False, target_theta=True, mix_old=True):
+        """The pose and the expression embedding of every driver frame: the first half of a driver frame (head-pose
+        regressor, pose algebra, expression encoder), captured, four frames in flight.  Returns (theta_embed, pose_embed):
+        theta_embed = (scale, rotation, translation), each (N,3), the form custome_target_theta_embed takes and
+        pred_target_srt has; pose_embed (N,E).  animate(theta_embed, pose_embed) with the same pose options renders the
+        frames forward(None, driver_images) renders.
+        The expression encoder reads the face aligned by the frame's *mixed* pose (infer.py:568-601), so pose_embed depends
+        on mix / mix_old and, with mix=True, on the current identity's source pose: encode with the options and the identity
+        the embeddings will be rendered with.  theta_embed is the regressed pose, independent of both; target_theta only
+        chooses the rendering warp and has no effect here."""
+        if self._state is None:
+            raise RuntimeError("encode() called before a source image was given")
+        n, frame = self._frames(driver_images)
+        pipe = self._driver_pipeline(mix, True, mix_old, encode=True)
+        srt = torch.empty((n, 9), dtype=torch.float32, device=self.device)
+        pose_embed = torch.empty((n, self.cfg.expr_channels), dtype=torch.float32, device=self.device)
+        keep = []
+        for i in range(n):
+            t = frame(i)
+            sl = pipe.submit(t, st=self._state).slot
+            so = sl.run.static_state
+            with torch.cuda.stream(sl.stream):
+                srt[i:i + 1].copy_(so.srt, non_blocking=True)
+                pose_embed[i:i + 1].copy_(so.target_pose_embed, non_blocking=True)
+                ev = torch.cuda.Event()
+                ev.record()
+            keep.append((t, ev))  # t is read by the slot's stream: kept from the allocator until the frame is done (see _render)
+            if i >= 2 * pipe.depth and keep[i - 2 * pipe.depth][1].query():
+                keep[i - 2 * pipe.depth] = None
+        pipe.drain()
+        return tuple(srt[:, k:k + 3].contiguous() for k in (0, 3, 6)), pose_embed
+
+    @torch.no_grad()
+    def animate(self, theta_embed, pose_embed, mix=False, target_theta=True, mix_old=True):
+        """Render N frames of the current identity from N poses and N expression embeddings, with no driver image:
+        theta_embed = (scale, rotation, translation), each (N,3) (encode's output, pred_target_srt's form), pose_embed (N,E).
+        Captured image-free frames (no head-pose regressor, no expression encoder), four in flight.  Returns
+        (list[PIL], img (N,3,H,W)) like forward and sets pred_target_theta, pred_target_srt (the supplied pose) and
+        target_pose_embed of the last frame.  Mismatched shapes raise ValueError, no source pass yet RuntimeError, before
+        anything is queued."""
+        E = self.cfg.expr_channels
+        if not isinstance(theta_embed, (tuple, list)) or len(theta_embed) != 3:
+            raise ValueError("theta_embed must be (scale, rotation, translation), each (N,3)")
+        parts = [torch.as_tensor(t) for t in theta_embed]
+        pose_embed = torch.as_tensor(pose_embed)
+        if pose_embed.dim() != 2 or pose_embed.shape[1] != E or pose_embed.shape[0] < 1:
+            raise ValueError(f"pose_embed must be (N,{E}) with N >= 1, got {tuple(pose_embed.shape)}")
+        n = pose_embed.shape[0]
+        if any(tuple(p.shape) != (n, 3) for p in parts):
+            raise ValueError(f"theta_embed must be three (N,3) tensors with N = {n} (pose_embed's), got "
+                             f"{[tuple(p.shape) for p in parts]}")
+        if self._state is None:
+            raise RuntimeError("animate() called before a source image was given")
+        srt = torch.cat([p.to(self.device).float() for p in parts], 1).contiguous()
+        pose_embed = pose_embed.to(self.device).float().contiguous()
+        pipe = self._driver_pipeline(mix, target_theta, mix_old, image=False, theta_embed=True, pose_embed=True)
+        return self._render(pipe, n, lambda i: dict(drv=None, theta_embed=srt[i:i + 1], pose_embed=pose_embed[i:i + 1]))
 
     # -- notebooks/infer.py:229-243
     def convert_to_tensor(self, image):
@@ -552,18 +707,22 @@ class InferenceWrapper(torch.nn.Module):
         custom_srt = None
         if custome_target_theta_embed is not None:   # (scale, rotation, translation), each (1,3): infer.py:566-567
             custom_srt = torch.cat([torch.as_tensor(t).float().reshape(1, 3) for t in custome_target_theta_embed], 1)
-        per_frame = smooth_pose or custom_srt is not None or custome_target_pose_embed is not None
-        if not per_frame and isinstance(driver_image, list) and len(driver_image) > 1 and not isinstance(driver_image[0], torch.Tensor):
-            return self._forward_list(driver_image, mix, target_theta, mix_old)
+        # one pose / embedding for every frame of the call; the captured frames read them from buffers of their own
+        embeds = dict(theta_embed=None if custom_srt is None else custom_srt.to(self.device).contiguous(),
+                      pose_embed=None if custome_target_pose_embed is None else
+                      torch.as_tensor(custome_target_pose_embed).to(self.device).float().reshape(1, -1).contiguous())
+        if not smooth_pose and isinstance(driver_image, list) and len(driver_image) > 1 and not isinstance(driver_image[0], torch.Tensor):
+            return self._forward_list(driver_image, mix, target_theta, mix_old, **embeds)
         drv = self._prep(driver_image)
-        if not per_frame:
+        if not smooth_pose:
             # captured driver frames (CUDA graphs), four in flight when a list of frames is given (DriverPipeline); same
-            # kernels as the eager pass below
-            self._driver_pipeline(mix, target_theta, mix_old)
+            # kernels as the eager pass below.  With a custom pose / embedding the graphs take it as an input; the
+            # expression encoder is then not captured, and pred_target_srt stays the regressed pose (infer.py:563-564)
+            pipe = self._driver_pipeline(mix, target_theta, mix_old, **{k: v is not None for k, v in embeds.items()})
             img = torch.empty_like(drv)
             for i in range(drv.shape[0]):
-                sl = self._pipeline.submit(drv[i:i + 1], dev_out=img[i:i + 1], st=self._state).slot
-            self._pipeline.drain()
+                sl = pipe.submit(drv[i:i + 1], dev_out=img[i:i + 1], st=self._state, **embeds).slot
+            pipe.drain()
             so = sl.run.static_state
             self.pred_target_theta = so.pred_target_theta.clone()
             self.pred_target_srt = (so.srt[:, :3].clone(), so.srt[:, 3:6].clone(), so.srt[:, 6:9].clone())
@@ -594,19 +753,18 @@ class InferenceWrapper(torch.nn.Module):
             self.pred_target_srt = (so.srt[:, :3].clone(), so.srt[:, 3:6].clone(), so.srt[:, 6:9].clone())
             self.target_pose_embed = so.target_pose_embed.clone()
         else:
+            # smooth_pose with a custom pose or embedding: eager frames.  self.theta is the smoothed (3,4) pose carried from
+            # frame to frame (infer.py:571-581); the device kernel seeds it with the first frame's pose and updates it in place
             imgs = []
             for i in range(drv.shape[0]):
-                kw = {}
-                if smooth_pose:
-                    # self.theta is the smoothed (3,4) pose carried from frame to frame (infer.py:571-581); the device
-                    # kernel seeds it with the first frame's pose and updates it in place
-                    init = self.theta is None
-                    if init:
-                        self.theta = torch.zeros((3, 4), dtype=torch.float32, device=self.device)
-                    kw = dict(smooth_state=self.theta, smooth_momentum=self.pose_momentum, smooth_init=init)
+                init = self.theta is None
+                if init:
+                    self.theta = torch.zeros((3, 4), dtype=torch.float32, device=self.device)
                 im, deep_f, img_f, so = self.model.driver_pass(self._state, drv[i:i + 1].contiguous(), mix=mix,
                                                                target_theta=target_theta, mix_old=mix_old, custom_srt=custom_srt,
-                                                               custom_pose_embed=custome_target_pose_embed, **kw)
+                                                               custom_pose_embed=custome_target_pose_embed,
+                                                               smooth_state=self.theta, smooth_momentum=self.pose_momentum,
+                                                               smooth_init=init)
                 imgs.append(im)
             img = imgs[0] if len(imgs) == 1 else torch.cat(imgs)
             self.pred_target_theta = so.pred_target_theta

@@ -41,11 +41,11 @@ N_IDS = (1, 2, 4, 8)
 
 
 def photo_to_photo_ms(wrapper, sources, drv, reps, recapture=False):
-    """median wall time of wrapper.forward(sources[i % n], drv); recapture: the wrapper's captured pipeline is dropped first"""
+    """median wall time of wrapper.forward(sources[i % n], drv); recapture: the wrapper's captured pipelines are dropped first"""
     out = []
     for i in range(reps):
         if recapture:
-            wrapper._pipeline = None
+            wrapper._pipelines.clear()
         torch.cuda.synchronize()
         t0 = time.perf_counter()
         wrapper.forward(sources[i % len(sources)], drv, crop=False, mix=True, mix_old=False)
