@@ -450,6 +450,30 @@ struct ResizeParams {
   float* out;
 };
 
+// One output pixel (n, oh, ow) of the bilinear resize, sh = Hin / Hout, sw = Win / Wout: for every channel c < C_pad,
+// emit(c, v) with v = post(c, interpolation of input channel c) for c < C and v = 0 above.  resize_bilinear_kernel and
+// s2_prepare_kernel both call it, so the stage-2 input is the same bits as emo_resize_bilinear's.
+template <class Post, class Emit>
+__device__ __forceinline__ void bilinear_pixel(const float* in, int n, int C, int C_pad, int Hin, int Win, int oh, int ow, float sh,
+                                               float sw, Post post, Emit emit) {
+  float sy = fmaxf(((float)oh + 0.5f) * sh - 0.5f, 0.f);
+  float sx = fmaxf(((float)ow + 0.5f) * sw - 0.5f, 0.f);
+  const int y0 = (int)sy, x0 = (int)sx;
+  const int y1 = y0 + (y0 < Hin - 1 ? 1 : 0), x1 = x0 + (x0 < Win - 1 ? 1 : 0);
+  const float ly = sy - (float)y0, lx = sx - (float)x0;
+  const float hy = 1.f - ly, hx = 1.f - lx;
+  for (int c = 0; c < C_pad; ++c) {
+    float acc = 0.f;
+    if (c < C) {
+      const float* s = in + ((long long)n * C + c) * Hin * Win;
+      acc = hy * (hx * __ldg(s + y0 * Win + x0) + lx * __ldg(s + y0 * Win + x1)) +
+            ly * (hx * __ldg(s + y1 * Win + x0) + lx * __ldg(s + y1 * Win + x1));
+      acc = post(c, acc);
+    }
+    emit(c, acc);
+  }
+}
+
 __global__ void resize_bilinear_kernel(const ResizeParams p) {
   const long long total = (long long)p.N * p.Hout * p.Wout;
   const float sh = (float)p.Hin / (float)p.Hout, sw = (float)p.Win / (float)p.Wout;
@@ -458,21 +482,87 @@ __global__ void resize_bilinear_kernel(const ResizeParams p) {
     const int ow = (int)(r % p.Wout); r /= p.Wout;
     const int oh = (int)(r % p.Hout); r /= p.Hout;
     const int n = (int)r;
-    float sy = fmaxf(((float)oh + 0.5f) * sh - 0.5f, 0.f);
-    float sx = fmaxf(((float)ow + 0.5f) * sw - 0.5f, 0.f);
-    const int y0 = (int)sy, x0 = (int)sx;
-    const int y1 = y0 + (y0 < p.Hin - 1 ? 1 : 0), x1 = x0 + (x0 < p.Win - 1 ? 1 : 0);
-    const float ly = sy - (float)y0, lx = sx - (float)x0;
-    const float hy = 1.f - ly, hx = 1.f - lx;
-    for (int c = 0; c < p.C_pad; ++c) {
-      float acc = 0.f;
-      if (c < p.C) {
-        const float* s = p.in + ((long long)n * p.C + c) * p.Hin * p.Win;
-        acc = hy * (hx * __ldg(s + y0 * p.Win + x0) + lx * __ldg(s + y0 * p.Win + x1)) +
-              ly * (hx * __ldg(s + y1 * p.Win + x0) + lx * __ldg(s + y1 * p.Win + x1));
-        if (p.mean) acc = (acc - __ldg(p.mean + c)) / __ldg(p.std + c);
-      }
-      p.out[idx * p.C_pad + c] = acc;
+    bilinear_pixel(p.in, n, p.C, p.C_pad, p.Hin, p.Win, oh, ow, sh, sw,
+                   [&](int c, float acc) {
+                     if (p.mean) acc = (acc - __ldg(p.mean + c)) / __ldg(p.std + c);
+                     return acc;
+                   },
+                   [&](int c, float acc) { p.out[idx * p.C_pad + c] = acc; });
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
+// the stage-1 -> stage-2 handoff of a refined frame (emo_s2_prepare, emo_s2_finish)
+// ------------------------------------------------------------------------------------------------
+// One CTA = kS2Tile consecutive output pixels of one row of one image.  Each pixel's bilinear value is computed once by
+// bilinear_pixel and written as the NCHW `resized` image and as the stem's operand: the channels-last (R, G, B, 0) pixel of
+// emo_resize_bilinear (C_pad 4), or (FP16) the 7 horizontal taps of emo_stem_pack's plane, packed by plane4_h from the tile's
+// values and a 3-pixel halo on each side, staged in shared memory.
+constexpr int kS2Tile = 256;
+
+template <bool FP16>
+__global__ void __launch_bounds__(kS2Tile) s2_prepare_kernel(const float* __restrict__ img, int Hin, int Win, int S, float sh, float sw,
+                                                              float* __restrict__ resized, float4* __restrict__ x4, uint4* __restrict__ plane,
+                                                              float scale) {
+  __shared__ float4 row[kS2Tile + 6];
+  const int tiles = (S + kS2Tile - 1) / kS2Tile;
+  const int w0 = (int)(blockIdx.x % tiles) * kS2Tile;
+  const int oh = (int)((blockIdx.x / tiles) % S);
+  const int n = (int)(blockIdx.x / ((long long)tiles * S));
+  const auto pixel = [&](int ow) {
+    float v[4];
+    bilinear_pixel(img, n, 3, 4, Hin, Win, oh, ow, sh, sw, [](int, float acc) { return acc; }, [&](int c, float acc) { v[c] = acc; });
+    return make_float4(v[0], v[1], v[2], v[3]);
+  };
+  const int ow = w0 + (int)threadIdx.x;
+  const long long HW = (long long)S * S;
+  const long long pix = (long long)n * HW + (long long)oh * S + ow;
+  if (FP16) {
+    for (int i = threadIdx.x; i < kS2Tile + 6; i += kS2Tile) {
+      const int x = w0 + i - 3;
+      row[i] = (x >= 0 && x < S) ? pixel(x) : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    __syncthreads();
+    if (ow >= S) return;
+    const float4 v = row[threadIdx.x + 3];
+    resized[(n * 3 + 0) * HW + (long long)oh * S + ow] = v.x;
+    resized[(n * 3 + 1) * HW + (long long)oh * S + ow] = v.y;
+    resized[(n * 3 + 2) * HW + (long long)oh * S + ow] = v.z;
+    uint2 t[8];
+#pragma unroll
+    for (int kx = 0; kx < 7; ++kx) {
+      const int ix = ow + kx - 3;
+      t[kx] = (ix >= 0 && ix < S) ? plane4_h(row[threadIdx.x + kx], scale) : make_uint2(0u, 0u);
+    }
+    t[7] = make_uint2(0u, 0u);
+    uint4* o = plane + pix * 4;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) o[j] = make_uint4(t[2 * j].x, t[2 * j].y, t[2 * j + 1].x, t[2 * j + 1].y);
+  } else {
+    if (ow >= S) return;
+    const float4 v = pixel(ow);
+    resized[(n * 3 + 0) * HW + (long long)oh * S + ow] = v.x;
+    resized[(n * 3 + 1) * HW + (long long)oh * S + ow] = v.y;
+    resized[(n * 3 + 2) * HW + (long long)oh * S + ow] = v.z;
+    x4[pix] = v;
+  }
+}
+
+// ffhq = clamp(resized + add, 0, 1) as torch computes it (one fp32 add, NaN kept), and its uint8 frame as image_to_u8_kernel
+// writes it (trunc(clamp(x, 0, 1) * 255), NaN -> 0): thread = one pixel of the 3-channel NCHW images.
+__global__ void __launch_bounds__(256) s2_finish_kernel(const float* __restrict__ resized, const float* __restrict__ add, int N, long long HW,
+                                                        float* __restrict__ out, unsigned char* __restrict__ u8) {
+  const long long total = (long long)N * HW;
+  for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (long long)gridDim.x * blockDim.x) {
+    const long long n = t / HW, s = t - n * HW;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      const long long i = (n * 3 + c) * HW + s;
+      const float x = __fadd_rn(__ldg(resized + i), __ldg(add + i));
+      const float y = x != x ? x : fminf(fmaxf(x, 0.f), 1.f);
+      out[i] = y;
+      const float v = fminf(fmaxf(y, 0.f), 1.f) * 255.f;
+      u8[t * 3 + c] = (unsigned char)(int)v;
     }
   }
 }
@@ -706,4 +796,35 @@ extern "C" int emo_resize_bilinear(const emo_resize_bilinear_desc* d, void* stre
   const long long total = (long long)d->N * d->Hout * d->Wout;
   launch_kernel(resize_bilinear_kernel, (unsigned)cdivll(total, 128), 128, 0, stream, p);
   return check_launch("emo_resize_bilinear");
+}
+
+extern "C" int emo_s2_prepare(const float* img, int N, int Hin, int Win, int S, float* resized, float* x4, void* plane, float plane_scale,
+                              void* stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  EMO_REQUIRE(img && resized, "emo_s2_prepare: null pointer");
+  EMO_REQUIRE((x4 != nullptr) != (plane != nullptr), "emo_s2_prepare: exactly one stem operand (x4 or plane) must be given");
+  EMO_REQUIRE(N > 0 && Hin > 0 && Win > 0 && S > 0, "emo_s2_prepare: bad shape (N=%d Hin=%d Win=%d S=%d)", N, Hin, Win, S);
+  EMO_REQUIRE(((uintptr_t)(x4 ? (const void*)x4 : plane) % 16) == 0, "emo_s2_prepare: the stem operand must be 16-byte aligned");
+  if (plane) EMO_REQUIRE(plane_scale > 0.f, "emo_s2_prepare: plane_scale must be positive");
+  const long long blocks = (long long)N * S * cdiv(S, kS2Tile);
+  EMO_REQUIRE(blocks < (1ll << 31), "emo_s2_prepare: grid too large");
+  const float sh = (float)Hin / (float)S, sw = (float)Win / (float)S;
+  if (plane)
+    launch_kernel(s2_prepare_kernel<true>, (unsigned)blocks, kS2Tile, 0, stream, img, Hin, Win, S, sh, sw, resized, (float4*)nullptr,
+                  (uint4*)plane, plane_scale);
+  else
+    launch_kernel(s2_prepare_kernel<false>, (unsigned)blocks, kS2Tile, 0, stream, img, Hin, Win, S, sh, sw, resized, (float4*)x4,
+                  (uint4*)nullptr, 0.f);
+  return check_launch("emo_s2_prepare");
+}
+
+extern "C" int emo_s2_finish(const float* resized, const float* add, int N, int H, int W, float* out, unsigned char* u8, void* stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  EMO_REQUIRE(resized && add && out && u8, "emo_s2_finish: null pointer");
+  EMO_REQUIRE(N > 0 && H > 0 && W > 0, "emo_s2_finish: bad shape (N=%d H=%d W=%d)", N, H, W);
+  const long long total = (long long)N * H * W;
+  long long blocks = cdivll(total, 256);
+  if (blocks > 132ll * 16) blocks = 132ll * 16;
+  launch_kernel(s2_finish_kernel, (unsigned)blocks, 256, 0, stream, resized, add, N, (long long)H * W, out, u8);
+  return check_launch("emo_s2_finish");
 }

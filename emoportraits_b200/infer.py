@@ -206,9 +206,19 @@ class Model:
         if encode and not (image and not theta_embed and not pose_embed):
             raise ValueError("an encoding frame reads a driver image and nothing else")
 
+    def check_refine(self, refine, encode: bool) -> None:
+        """ValueError unless `refine` (a stage2.Stage2Model or None) can follow this model's frames in one graph"""
+        if refine is None:
+            return
+        if encode:
+            raise ValueError("an encoding frame renders no image to refine: refine needs encode=False")
+        if ops._dev_key(refine.device) != ops._dev_key(self.device):
+            raise ValueError(f"the stage-2 model is on {refine.device}, the stage-1 model on {self.device}: refined frames run "
+                             "both on one device")
+
     def make_driver_graph(self, st, mix: bool = True, target_theta: bool = True, slot: int = 0, mix_old: bool = False,
                           smooth_state: Optional[torch.Tensor] = None, smooth_momentum: float = 0.5, image: bool = True,
-                          theta_embed: bool = False, pose_embed: bool = False, encode: bool = False):
+                          theta_embed: bool = False, pose_embed: bool = False, encode: bool = False, refine=None):
         """Capture one driver frame (all ~240 kernel launches) into a CUDA graph: removes the Python/ctypes launch
         overhead from the per-frame loop.  Returns replay(drv (1,3,H,W) on device) -> img (1,3,H,W) (static buffer).
         The graph reads its identity from buffers of its own (replay.identity, dist.new_identity), never from `st`:
@@ -224,17 +234,22 @@ class Model:
         expression embedding (the expression encoder is then not captured).  Without an image the head-pose regressor is
         not captured either.  encode: the graph stops after the expression encoder (driver_pass(encode_only=True)):
         replay.static_state.srt / .target_pose_embed are the frame's pose and embedding, static_out is None, and its
-        identity buffers hold only the source pose, the one identity field the embedding depends on."""
+        identity buffers hold only the source pose, the one identity field the embedding depends on.
+        refine (a stage2.Stage2Model on this device): the graph continues with stage 2 on the frame's image
+        (Stage2Model.refine, the stage-2 wrapper's default masks): replay.static_out is then the refined (1,3,S2,S2) image,
+        replay.static_u8 its (1,S2,S2,3) uint8 frame and replay.static_stage1 the stage-1 image.  The warm-up passes run
+        stage 2 under the same scratch set, so its workspaces exist before the capture."""
         self.check_inputs(image, theta_embed, pose_embed, encode)
+        self.check_refine(refine, encode)
         prev = ops.set_slot(slot)
         try:
             return self._make_driver_graph(st, mix, target_theta, mix_old, smooth_state, smooth_momentum, image, theta_embed,
-                                           pose_embed, encode)
+                                           pose_embed, encode, refine)
         finally:
             ops.set_slot(prev)
 
     def _make_driver_graph(self, st, mix, target_theta, mix_old=False, smooth_state=None, smooth_momentum=0.5, image=True,
-                           theta_embed=False, pose_embed=False, encode=False):
+                           theta_embed=False, pose_embed=False, encode=False, refine=None):
         s, dev = self.cfg.image_size, self.device
         static_in = torch.zeros((1, 3, s, s), dtype=torch.float32, device=dev) if image else None
         # the warm-up passes run on the unit pose (scale 1, no rotation or translation) and a zero embedding
@@ -278,19 +293,25 @@ class Model:
         side.wait_stream(torch.cuda.current_stream(self.device))
         with torch.cuda.stream(side):
             for _ in range(2):
-                self.driver_pass(identity, static_in, **kw)
+                img = self.driver_pass(identity, static_in, **kw)[0]
+                if refine is not None:
+                    refine.refine(img)
         torch.cuda.current_stream(self.device).wait_stream(side)
         torch.cuda.synchronize(self.device)
         graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(graph):
             out = self.driver_pass(identity, static_in, **kw)
-            static_out = out[0]
+            static_out = static_stage1 = out[0]
+            static_u8 = None
+            if refine is not None:
+                _, static_out, static_u8 = refine.refine(static_stage1)
         if smooth_state is not None:
             smooth_state.copy_(saved)
 
         replay.graph = graph
         replay.static_in, replay.static_out, replay.static_state = static_in, static_out, out[3]
         replay.static_theta, replay.static_pose = static_theta, static_pose
+        replay.static_stage1, replay.static_u8 = static_stage1, static_u8
         return replay
 
 
@@ -310,18 +331,24 @@ class DriverPipeline:
 
     image / theta_embed / pose_embed name the inputs every frame takes (Model.make_driver_graph): the driver image, and the
     caller's pose (1,9) and expression embedding (1,E) for the frame.  encode: each frame stops after the expression
-    encoder; its pose and embedding are slot.run.static_state.srt / .target_pose_embed."""
+    encoder; its pose and embedding are slot.run.static_state.srt / .target_pose_embed.
+
+    refine (a stage2.Stage2Model): every frame is refined by stage 2 in the same graph (Model.make_driver_graph):
+    slot.run.static_out is the refined (1,3,S2,S2) image, slot.run.static_u8 its uint8 frame and slot.run.static_stage1 the
+    stage-1 image.  submit(..., u8_out=) copies the uint8 frame out on the frame's stream."""
 
     def __init__(self, model: "Model", st, depth: int = 2, mix: bool = True, target_theta: bool = True, mix_old: bool = False,
-                 image: bool = True, theta_embed: bool = False, pose_embed: bool = False, encode: bool = False):
+                 image: bool = True, theta_embed: bool = False, pose_embed: bool = False, encode: bool = False, refine=None):
         model.check_inputs(image, theta_embed, pose_embed, encode)
+        model.check_refine(refine, encode)
         self.model, self.depth, self.n = model, depth, 0
         self.image, self.theta_embed, self.pose_embed, self.encode = image, theta_embed, pose_embed, encode
+        self.refine = refine
         self.st = st  # the current identity: frames submitted without st= animate it
         self.slots = []
         for k in self.scratch_slots(depth):
             run = model.make_driver_graph(st, mix=mix, target_theta=target_theta, slot=k, mix_old=mix_old, image=image,
-                                          theta_embed=theta_embed, pose_embed=pose_embed, encode=encode)
+                                          theta_embed=theta_embed, pose_embed=pose_embed, encode=encode, refine=refine)
             self.slots.append(SimpleNamespace(run=run, stream=torch.cuda.Stream(device=model.device),
                                               done=torch.cuda.Event(), busy=False))
 
@@ -331,8 +358,17 @@ class DriverPipeline:
         (Model.source_pass / driver_pass on the current stream), which may overlap frames in flight."""
         return [k + 1 for k in range(depth)]
 
-    def _check_submit(self, drv, theta_embed, pose_embed, outs) -> None:
-        """ValueError unless a frame's inputs are the ones the pipeline was captured for, of the right shapes"""
+    def _check_submit(self, drv, theta_embed, pose_embed, outs, u8_out=None) -> None:
+        """ValueError unless a frame's inputs are the ones the pipeline was captured for, of the right shapes, and u8_out
+        a (1,S2,S2,3) uint8 buffer of a refining pipeline"""
+        if u8_out is not None:
+            if self.refine is None:
+                raise ValueError("u8_out: only a refining pipeline (refine=) writes a uint8 frame")
+            s2 = self.refine.cfg.output_size
+            if not isinstance(u8_out, torch.Tensor) or tuple(u8_out.shape) != (1, s2, s2, 3) or u8_out.dtype != torch.uint8 \
+                    or not u8_out.is_contiguous():
+                got = (tuple(u8_out.shape), u8_out.dtype) if isinstance(u8_out, torch.Tensor) else type(u8_out).__name__
+                raise ValueError(f"u8_out must be a contiguous uint8 tensor of shape {(1, s2, s2, 3)}, got {got}")
         given = dict(image=drv is not None, theta_embed=theta_embed is not None, pose_embed=pose_embed is not None)
         want = dict(image=self.image, theta_embed=self.theta_embed, pose_embed=self.pose_embed)
         if given != want:
@@ -347,7 +383,8 @@ class DriverPipeline:
             raise ValueError("an encoding pipeline renders no image: host_out / dev_out must be None")
 
     def submit(self, drv: Optional[torch.Tensor], host_out: Optional[torch.Tensor] = None, dev_out: Optional[torch.Tensor] = None,
-               st=None, theta_embed: Optional[torch.Tensor] = None, pose_embed: Optional[torch.Tensor] = None):
+               st=None, theta_embed: Optional[torch.Tensor] = None, pose_embed: Optional[torch.Tensor] = None,
+               u8_out: Optional[torch.Tensor] = None):
         """Queue one frame (device tensor, or pinned host tensor -> asynchronous H2D on the frame's stream).  If `host_out`
         (pinned) / `dev_out` is given the image is copied into it on the same stream.  Returns a ticket: ticket.done is an
         event recorded when this frame (and its copy-out) has finished (ticket.slot.done is the same event, i.e. always the
@@ -359,10 +396,12 @@ class DriverPipeline:
         state whose source pass was just queued there may be given at once, and the caller may drop it after this call.
         theta_embed (1,9) / pose_embed (1,E): the frame's pose and expression embedding, for a pipeline captured to take
         them; they are copied into the slot's buffers on its stream like the image.  drv is None for an image-free
-        pipeline.  Inputs other than the pipeline's, or of other shapes, raise ValueError before anything is queued."""
+        pipeline.  Inputs other than the pipeline's, or of other shapes, raise ValueError before anything is queued.
+        u8_out (1,S2,S2,3) uint8, pinned host or device (a refining pipeline only): the refined frame's uint8 image
+        (slot.run.static_u8) is copied into it on the frame's stream, before ticket.done."""
         if st is not None:
             check_identity(st, self.model.cfg)
-        self._check_submit(drv, theta_embed, pose_embed, (host_out, dev_out))
+        self._check_submit(drv, theta_embed, pose_embed, (host_out, dev_out), u8_out)
         if st is not None:
             self.st = st
         sl = self.slots[self.n % self.depth]
@@ -380,6 +419,8 @@ class DriverPipeline:
                 host_out.copy_(sl.run.static_out, non_blocking=True)
             if dev_out is not None:
                 dev_out.copy_(sl.run.static_out, non_blocking=True)
+            if u8_out is not None:
+                u8_out.copy_(sl.run.static_u8, non_blocking=True)
             sl.done = torch.cuda.Event()
             sl.done.record()
         sl.busy = True
@@ -502,14 +543,22 @@ class InferenceWrapper(torch.nn.Module):
     # rendering); the least recently used is dropped for a new one.  Plain frames, encode(), animate() and forward with an
     # embedding then alternate with no capture.
     PIPELINES = 4
+    # Frames in flight of a refining pipeline (forward_refined).  Stage 2 at batch 1 @1024^2 fills an H100 on its own:
+    # two, three and four frames in flight run within 1 % of each other (tools/refine_stream_bench.py, DESIGN.md section 7),
+    # while every slot holds ~4 GB (exact) of captured activations.  Two keep one frame's host-side work under the other's.
+    REFINE_DEPTH = 2
 
-    def _driver_pipeline(self, mix, target_theta, mix_old, **inputs):
-        """the captured four-in-flight pipeline of these options (DriverPipeline's image / theta_embed / pose_embed / encode);
-        it serves every identity (submit(..., st=))"""
+    def _driver_pipeline(self, mix, target_theta, mix_old, refine=None, **inputs):
+        """the captured four-in-flight pipeline of these options (DriverPipeline's image / theta_embed / pose_embed / encode,
+        and the stage-2 model that refines its frames, keyed with its precision); it serves every identity (submit(..., st=))"""
         key = (bool(mix), bool(target_theta), bool(mix_old), tuple(sorted(inputs.items())))
+        if refine is not None:
+            key += (("refine", refine, refine.precision),)
         pipe = self._pipelines.pop(key, None)
         if pipe is None:
-            pipe = DriverPipeline(self.model, self._state, depth=4, mix=mix, target_theta=target_theta, mix_old=mix_old, **inputs)
+            depth = 4 if refine is None else self.REFINE_DEPTH
+            pipe = DriverPipeline(self.model, self._state, depth=depth, mix=mix, target_theta=target_theta, mix_old=mix_old,
+                                  refine=refine, **inputs)
         self._pipelines[key] = pipe
         # the new pipeline's captures synchronized the device, so nothing of a dropped one is still running
         while len(self._pipelines) > self.PIPELINES:
@@ -528,23 +577,29 @@ class InferenceWrapper(torch.nn.Module):
 
     def _render(self, pipe, n, inputs):
         """n frames through `pipe`, frame i with the submit arguments inputs(i), returned as forward returns them; sets the
-        pred_target_* attributes from the last frame"""
+        pred_target_* attributes from the last frame.  A refining pipeline's frames are its refined images, whose uint8
+        frames the graph wrote: they are copied straight into the pinned host buffer."""
         from PIL import Image
 
-        s = self.cfg.image_size
+        refine = getattr(pipe, "refine", None)
+        s = self.cfg.image_size if refine is None else refine.cfg.output_size
         img = torch.empty((n, 3, s, s), dtype=torch.float32, device=self.device)
-        u8 = torch.empty((n, s, s, 3), dtype=torch.uint8, device=self.device)
+        u8 = torch.empty((n, s, s, 3), dtype=torch.uint8, device=self.device) if refine is None else None
         host = torch.empty((n, s, s, 3), dtype=torch.uint8).pin_memory()
         keep, done = [], []
         for i in range(n):
             kw = inputs(i)
             keep.append(kw)  # read by the slot's stream later: must not return to the allocator (of the current stream) before
-            sl = pipe.submit(dev_out=img[i:i + 1], st=self._state, **kw).slot
-            with torch.cuda.stream(sl.stream):
-                ops.image_to_u8(img[i:i + 1], out=u8[i:i + 1])  # clamp(0, 1) + ToPILImage (mul(255).byte()) on the device
-                host[i].copy_(u8[i], non_blocking=True)
-                ev = torch.cuda.Event()
-                ev.record()
+            if refine is not None:
+                t = pipe.submit(dev_out=img[i:i + 1], u8_out=host[i:i + 1], st=self._state, **kw)
+                sl, ev = t.slot, t.done
+            else:
+                sl = pipe.submit(dev_out=img[i:i + 1], st=self._state, **kw).slot
+                with torch.cuda.stream(sl.stream):
+                    ops.image_to_u8(img[i:i + 1], out=u8[i:i + 1])  # clamp(0, 1) + ToPILImage (mul(255).byte()) on the device
+                    host[i].copy_(u8[i], non_blocking=True)
+                    ev = torch.cuda.Event()
+                    ev.record()
             done.append(ev)
             if len(keep) > 2 * pipe.depth and done[i - 2 * pipe.depth].query():
                 keep[i - 2 * pipe.depth] = None
@@ -625,6 +680,66 @@ class InferenceWrapper(torch.nn.Module):
         pose_embed = pose_embed.to(self.device).float().contiguous()
         pipe = self._driver_pipeline(mix, target_theta, mix_old, image=False, theta_embed=True, pose_embed=True)
         return self._render(pipe, n, lambda i: dict(drv=None, theta_embed=srt[i:i + 1], pose_embed=pose_embed[i:i + 1]))
+
+    @staticmethod
+    def _theta_rows(theta_embed) -> torch.Tensor:
+        """(scale, rotation, translation), each (N,3), as one (N,9) tensor (ValueError otherwise)"""
+        if not isinstance(theta_embed, (tuple, list)) or len(theta_embed) != 3:
+            raise ValueError("theta_embed must be (scale, rotation, translation), each (N,3)")
+        parts = [torch.as_tensor(t).float() for t in theta_embed]
+        if any(p.dim() != 2 or p.shape[1] != 3 or p.shape[0] != parts[0].shape[0] for p in parts) or parts[0].shape[0] < 1:
+            raise ValueError(f"theta_embed must be three (N,3) tensors with one N >= 1, got {[tuple(p.shape) for p in parts]}")
+        return torch.cat([p.cpu() for p in parts], 1)
+
+    @torch.no_grad()
+    def forward_refined(self, driver_images, inferer_s2, mix=False, target_theta=True, mix_old=True,
+                        custome_target_theta_embed=None, custome_target_pose_embed=None):
+        """Driver frames refined by stage 2, each in one captured graph: the stage-1 frame, then inferer_s2's stage 2
+        (a stage2.InferenceWrapper on this device, with its default masks) on its image, REFINE_DEPTH frames in flight.
+        The refining pipeline is cached with the others (PIPELINES), keyed by the stage-2 model and its precision.
+        driver_images: what forward's driver path takes (a list of PIL / numpy frames, converted as each is queued; a tensor
+        batch; one image), with custome_target_theta_embed / custome_target_pose_embed as in forward (one pose / embedding
+        for every frame).  driver_images=None with both embeddings: frames rendered from them as animate renders them,
+        theta_embed (N,3) x 3 and pose_embed (N,E).  Returns (list[PIL] of the refined S2 x S2 frames, img (N,3,S2,S2) on
+        the device); frame i is inferer_s2.forward(self.forward(None, frame_i, ...)[1])[2][0].  Sets pred_target_theta,
+        pred_target_srt and target_pose_embed of the last frame.  There is no smooth_pose form: smoothing is a recurrence
+        over the frames, which this path does not run.  Refused before anything is queued: no source pass yet
+        (RuntimeError), a stage-2 wrapper on another device or inputs that do not fit (ValueError)."""
+        if self._state is None:
+            raise RuntimeError("forward_refined() called before a source image was given")
+        s2 = getattr(inferer_s2, "model_two", None)
+        if s2 is None:
+            raise ValueError("inferer_s2 must be a stage2.InferenceWrapper")
+        self.model.check_refine(s2, encode=False)
+        E = self.cfg.expr_channels
+        if driver_images is None:
+            if custome_target_theta_embed is None or custome_target_pose_embed is None:
+                raise ValueError("forward_refined(None, ...) renders from custome_target_theta_embed and custome_target_pose_embed: "
+                                 "give both, or driver images")
+            srt = self._theta_rows(custome_target_theta_embed)
+            pe = torch.as_tensor(custome_target_pose_embed).float()
+            if pe.dim() != 2 or tuple(pe.shape) != (srt.shape[0], E):
+                raise ValueError(f"custome_target_pose_embed must be ({srt.shape[0]},{E}) (one row per pose), got {tuple(pe.shape)}")
+            srt, pe = srt.to(self.device).contiguous(), pe.to(self.device).contiguous()
+            pipe = self._driver_pipeline(mix, target_theta, mix_old, refine=s2, image=False, theta_embed=True, pose_embed=True)
+            return self._render(pipe, srt.shape[0], lambda i: dict(drv=None, theta_embed=srt[i:i + 1], pose_embed=pe[i:i + 1]))
+        if isinstance(driver_images, list) and not driver_images:
+            raise ValueError("forward_refined: no driver frame")
+        srt = pe = None
+        if custome_target_theta_embed is not None:
+            srt = self._theta_rows(custome_target_theta_embed)
+            if srt.shape[0] != 1:
+                raise ValueError("with driver images custome_target_theta_embed is one pose (1,3) x 3 for every frame")
+            srt = srt.to(self.device).contiguous()
+        if custome_target_pose_embed is not None:
+            pe = torch.as_tensor(custome_target_pose_embed).float()
+            if pe.numel() != E:
+                raise ValueError(f"with driver images custome_target_pose_embed is one embedding of {E} values for every frame, "
+                                 f"got {tuple(pe.shape)}")
+            pe = pe.to(self.device).reshape(1, E).contiguous()
+        n, frame = self._frames(driver_images)
+        pipe = self._driver_pipeline(mix, target_theta, mix_old, refine=s2, theta_embed=srt is not None, pose_embed=pe is not None)
+        return self._render(pipe, n, lambda i: dict(drv=frame(i), theta_embed=srt, pose_embed=pe))
 
     # -- notebooks/infer.py:229-243
     def convert_to_tensor(self, image):

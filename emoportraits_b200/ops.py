@@ -686,6 +686,40 @@ def image_to_u8(img_nchw: torch.Tensor, out: Optional[torch.Tensor] = None) -> t
     return out
 
 
+def s2_prepare(img_nchw: torch.Tensor, size: int, fast: bool):
+    """The stage-2 input of a stage-1 image (N,3,h,w) fp32 in one pass: (resized (N,3,S,S) fp32 NCHW, the stem's operand).
+    resized is resize_bilinear(img, (S, S)) as NCHW; the operand is that resize_bilinear output (N,1,S,S,4) itself, or with
+    `fast` stem_pack() of it (one fp16 plane (N,1,S,S,32)).  Same bits as the two-step path."""
+    _chk(img_nchw)
+    N, Cc, Hi, Wi = img_nchw.shape
+    assert Cc == 3, img_nchw.shape
+    resized = torch.empty((N, 3, size, size), dtype=torch.float32, device=img_nchw.device)
+    if fast:
+        stem_in = Split.empty((N, 1, size, size, STEM_CIN), img_nchw.device, H1)
+        x4, plane, scale = None, stem_in.hi, stem_in.scale
+    else:
+        stem_in = x4 = torch.empty((N, 1, size, size, 4), dtype=torch.float32, device=img_nchw.device)
+        plane, scale = None, 0.0
+    L.call("emo_s2_prepare", _p(img_nchw), N, Hi, Wi, size, _p(resized), _p(x4), _p(plane), C.c_float(scale), _stream())
+    return resized, stem_in
+
+
+def s2_finish(resized: torch.Tensor, add: torch.Tensor, out: Optional[torch.Tensor] = None,
+              u8: Optional[torch.Tensor] = None):
+    """(ffhq, u8): ffhq = (resized + add).clamp_(0, 1) (N,3,H,W) fp32 and u8 = image_to_u8(ffhq) (N,H,W,3), in one pass"""
+    _chk(resized); _chk(add)
+    N, Cc, H, W = resized.shape
+    assert Cc == 3 and add.shape == resized.shape, (resized.shape, add.shape)
+    if out is None:
+        out = torch.empty_like(resized)
+    if u8 is None:
+        u8 = torch.empty((N, H, W, 3), dtype=torch.uint8, device=resized.device)
+    _chk(out); _chk(u8, torch.uint8)
+    assert out.shape == resized.shape and tuple(u8.shape) == (N, H, W, 3), (out.shape, u8.shape)
+    L.call("emo_s2_finish", _p(resized), _p(add), N, H, W, _p(out), _p(u8), _stream())
+    return out, u8
+
+
 def resize_bicubic(img_nchw: torch.Tensor, out_hw) -> torch.Tensor:
     """F.interpolate(mode='bicubic', align_corners=False) (notebooks/infer.py:399-403, 551-556)"""
     _chk(img_nchw)

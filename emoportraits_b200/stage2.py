@@ -187,10 +187,14 @@ class Stage2Model:
     @torch.no_grad()
     def local_encoder(self, x4):
         """x4 (N,1,S,S,4) channels-last (masked, resized) image -> latent (N,1,64,64,C*depth)"""
+        return self._encode(ops.stem_pack(x4) if self.stem_h1 is not None else x4)
+
+    def _encode(self, stem_in):
+        """local_encoder from the stem's operand: x4 itself (exact) or its stem_pack plane (fast)"""
         if self.stem_h1 is not None:
-            x = ops.conv_igemm(ops.stem_pack(x4), self.stem_h1, pad=(0, 3, 0), bias=self.stem_b)
+            x = ops.conv_igemm(stem_in, self.stem_h1, pad=(0, 3, 0), bias=self.stem_b)
         else:
-            x = ops.conv_direct(x4, self.stem_w, 1, 3, self.stem_b)
+            x = ops.conv_direct(stem_in, self.stem_w, 1, 3, self.stem_b)
         for blk in self.enc:
             x, _ = blk(x, down=(1, 2, 2))
         a = ops.apply(x, **self.fin_norm.apply_args(), act=ops.ACT_RELU, planes=self.planes)
@@ -231,6 +235,18 @@ class Stage2Model:
         add = add * fm if not isinstance(fm, float) else add
         ffhq = (resized + add).clamp_(min=0, max=1)
         return resized, add, ffhq
+
+    @torch.no_grad()
+    def refine(self, img: torch.Tensor, out: Optional[torch.Tensor] = None, u8: Optional[torch.Tensor] = None):
+        """forward(img)'s ffhq without masks, as kernels only, so that a CUDA graph can capture it after a stage-1 frame:
+        ops.s2_prepare (the resize and the stem's operand in one pass) -> the encoder and decoder convolutions forward
+        runs -> ops.s2_finish (clamp(resized + add, 0, 1) and its uint8 frame in one pass).  img (N,3,h,w) fp32 contiguous
+        on the device.  out (N,3,S,S) fp32 / u8 (N,S,S,3) uint8: written in place if given.  Returns (resized, ffhq, u8),
+        bit-identical to forward(img)'s resized and ffhq and to ops.image_to_u8(ffhq)."""
+        resized, stem_in = ops.s2_prepare(img, self.cfg.output_size, fast=self.stem_h1 is not None)
+        add = self.decoder(self._encode(stem_in))
+        ffhq, u8 = ops.s2_finish(resized, add, out=out, u8=u8)
+        return resized, ffhq, u8
 
 
 class InferenceWrapper(torch.nn.Module):

@@ -35,7 +35,7 @@ extern "C" {
 enum { EMO_ACT_NONE = 0, EMO_ACT_RELU = 1, EMO_ACT_SIGMOID = 2, EMO_ACT_TANH = 3 };
 
 const char* emo_last_error(void);
-int emo_version(void); /* 107: + emo_stem_pack; 106: one-plane fp16 operands (emo_conv_desc, emo_apply_desc, emo_grid_sample3d_desc.plane_fp16,
+int emo_version(void); /* 108: + emo_s2_prepare, emo_s2_finish; 107: + emo_stem_pack; 106: one-plane fp16 operands (emo_conv_desc, emo_apply_desc, emo_grid_sample3d_desc.plane_fp16,
                           emo_split_f16 with lo == NULL) and the EMO_CONV_KERNEL_H1_* kernels; 105: + emo_conv_plan; 104: + emo_composite; 103: emo_conv_desc.post; 102: + emo_u8_to_image, emo_image_to_u8, emo_resize_bicubic; 101: emo_pose_desc and emo_conv_desc gained trailing fields */
 /* sm count, and cc major*10+minor of the current device */
 int emo_device_info(int* sm_count, int* cc);
@@ -399,6 +399,18 @@ int emo_split_f16(const float* x, long long n, float scale, void* hi, void* lo, 
 int emo_u8_to_image(const unsigned char* nhwc, int N, int H, int W, int C, float* nchw, void* stream);
 int emo_image_to_u8(const float* nchw, int N, int C, int H, int W, unsigned char* nhwc, void* stream);
 int emo_resize_bicubic(const float* in, int N, int C, int Hin, int Win, int Hout, int Wout, float* out, void* stream);
+/* The stage-1 -> stage-2 handoff of a refined frame (notebooks/infer_s2.py:351-376 on the stage-1 image), one pass each side.
+ *   emo_s2_prepare  img fp32 [N][3][Hin][Win] -> resized fp32 [N][3][S][S], the bilinear resize (align_corners=False) with the
+ *                   bits of emo_resize_bilinear, and the stage-2 stem's operand, exactly one of:
+ *                     x4     fp32 [N][S][S][4] = (R, G, B, 0), emo_resize_bilinear's output with C_pad 4 (the exact mode's
+ *                            emo_conv_direct input), 16-byte aligned;
+ *                     plane  fp16 [N][S][S][32], emo_stem_pack's plane of that x4 with scale plane_scale > 0 (the fast mode's
+ *                            7x1 implicit-GEMM operand), 16-byte aligned.
+ *   emo_s2_finish   resized, add fp32 [N][3][H][W] -> out fp32 [N][3][H][W] = clamp(resized + add, 0, 1) (one fp32 add, a NaN
+ *                   stays NaN, as torch's clamp) and u8 uint8 [N][H][W][3], emo_image_to_u8 of out. */
+int emo_s2_prepare(const float* img, int N, int Hin, int Win, int S, float* resized, float* x4, void* plane, float plane_scale,
+                   void* stream);
+int emo_s2_finish(const float* resized, const float* add, int N, int H, int W, float* out, unsigned char* u8, void* stream);
 /* Foreground / background compositing of the video loop (notebooks/E_emo_infer_video.ipynb cell 41, connect_img_and_bg):
  *   m' = (mask > threshold ? mask : 0)^8;  out = m' * img + (1 - m') * bg
  * img, out fp32 [N][C][H][W]; mask fp32 [N][1][H][W]; bg fp32 [C][H][W] (one background for the whole clip). */
