@@ -77,6 +77,9 @@ struct ConvKParams {
   // k-chunk) group is ONE halo tile of a_rows = tw * (th + kh - 1) pixels serving all kh tap rows; A ring of `sa` halo tiles,
   // B ring of `sb` weight tiles (see the kernel's producer role)
   int yreuse, sa, sb, a_rows;
+  // 1: every tile of the launch starts at channel 0 (one channel tile, ntc == 1), so the bias (x 1 / out_scale) is read once
+  // per CTA into kMaxBN floats of shared memory above the planned area, instead of from global memory by every tile
+  int bias_smem;
 };
 
 // ------------------------------------------------------------------------------------------------
@@ -254,6 +257,7 @@ conv_igemm_kernel(const __grid_constant__ TMaps tm, const __grid_constant__ Conv
   // are plain stores summed in a fixed order afterwards (no atomics inside the CTA: reproducible run to run)
   float* col_sum = (float*)(aempty_bar + kMaxAStages);  // [kConsumerWarps][kMaxBN]
   float* col_sq = col_sum + kConsumerWarps * kMaxBN;     // [kConsumerWarps][kMaxBN]
+  float* sbias = col_sq + kConsumerWarps * kMaxBN;       // [kMaxBN], p.bias_smem only: zero beyond Cout
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -277,6 +281,10 @@ conv_igemm_kernel(const __grid_constant__ TMaps tm, const __grid_constant__ Conv
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");  // every initialising lane publishes its own barriers
   }
   for (int i = threadIdx.x; i < 2 * kConsumerWarps * kMaxBN; i += kThreads) col_sum[i] = 0.f;
+  if (p.bias_smem && threadIdx.x < kMaxBN) {
+    const float binv = F16 ? 1.f / p.out_scale : 1.f;  // as the per-tile read below
+    sbias[threadIdx.x] = threadIdx.x < BN && (int)threadIdx.x < p.Cout ? __ldg(p.bias + threadIdx.x) * binv : 0.f;
+  }
   __syncthreads();
   EMO_STAMP(1, threadIdx.x == 0);
   const int tile_first = (int)blockIdx.x;
@@ -512,6 +520,17 @@ conv_igemm_kernel(const __grid_constant__ TMaps tm, const __grid_constant__ Conv
       pix = (long long)n * p.Dout * oHt * oWt + spi;
       rpix = p.residual ? (((long long)n * p.rD + od) * p.rH + (oh >> p.res_shift)) * p.rW + (ow >> p.res_shift) : 0;
     };
+    // this thread's columns of pixel `pix` of src (residual or post-add) into dst[0 .. BN/4), zero where src or the column
+    // does not exist (the even-channel final phase: both columns of a pair exist, 8-byte aligned)
+    auto load_pairs = [&](float* dst, const float* src, long long pix, bool valid) {
+#pragma unroll
+      for (int j = 0; j < kMaxBN / 8; ++j) {
+        const int c = n0 + 8 * j + cq;
+        float2 v = make_float2(0.f, 0.f);
+        if (8 * j < BN && src && valid && c < p.Cout && !EMO_DBG(4)) v = __ldg((const float2*)(src + pix * p.Cout + c));
+        dst[2 * j] = v.x; dst[2 * j + 1] = v.y;
+      }
+    };
     if (ksplit == 1 && (lane & 3) == 0 && (p.residual || p.post_add)) {
       // the residual / post-add rows are first read after this tile's main loop: pull them into L2 now
       const int nb = (BN < p.Cout - n0 ? BN : p.Cout - n0) * 4;
@@ -540,8 +559,13 @@ conv_igemm_kernel(const __grid_constant__ TMaps tm, const __grid_constant__ Conv
         const int c = n0 + 8 * j + cq;
         float b0 = 0.f, b1 = 0.f;
         if (8 * j < BN) {
-          if (c < p.Cout) b0 = __ldg(p.bias + c) * binv;
-          if (c + 1 < p.Cout) b1 = __ldg(p.bias + c + 1) * binv;
+          if (p.bias_smem) {
+            const float2 b = *(const float2*)(sbias + c);  // n0 == 0
+            b0 = b.x; b1 = b.y;
+          } else {
+            if (c < p.Cout) b0 = __ldg(p.bias + c) * binv;
+            if (c + 1 < p.Cout) b1 = __ldg(p.bias + c + 1) * binv;
+          }
         }
         acc[4 * j] = b0; acc[4 * j + 1] = b1; acc[4 * j + 2] = b0; acc[4 * j + 3] = b1;
       }
@@ -638,74 +662,96 @@ conv_igemm_kernel(const __grid_constant__ TMaps tm, const __grid_constant__ Conv
       constexpr bool pairs = decltype(pairs_c)::value;  // c even, Cout even: both columns of a pair exist, 8-byte aligned
       constexpr int act_k = decltype(act_c)::value;
       const int act = act_k >= 0 ? act_k : p.act;  // -1: the activation is read at run time (the scalar path)
+      if constexpr (pairs) {
+        // The residual / post-add values are loaded before the stores they precede: a load may not move over a store that may
+        // alias it, so a load after a store waits out a full memory latency.  They go to the chunk registers, which are free
+        // until the next tile's main loop: both rows' residual at once when there is no post-add (every residual layer of the
+        // models), otherwise one row's residual and post-add at a time.
+        bool valid[2];
+        long long pix[2], rpix[2], spi[2];
 #pragma unroll
-      for (int rr = 0; rr < 2; ++rr) {
-        bool valid;
-        long long pix, rpix, spi;
-        locate(rr, valid, pix, rpix, spi);
-        // the row's residual / post-add values are loaded together before any store (a load may not move over a store that
-        // may alias it, so loads interleaved with the stores would each wait out a full memory latency); they are kept in the
-        // chunk registers, which are free until the next tile's main loop
-#pragma unroll
-        for (int j = 0; j < kMaxBN / 8; ++j) {
-          const int c = n0 + 8 * j + cq;
-          float2 r2 = make_float2(0.f, 0.f), p2 = make_float2(0.f, 0.f);
-          if (8 * j < BN && pairs && valid && c < p.Cout && !EMO_DBG(4)) {
-            if (p.residual) r2 = __ldg((const float2*)(p.residual + rpix * p.Cout + c));
-            if (p.post_add) p2 = __ldg((const float2*)(p.post_add + spi * p.Cout + c));
-          }
-          cf[2 * j] = r2.x; cf[2 * j + 1] = r2.y; cf[kMaxBN / 4 + 2 * j] = p2.x; cf[kMaxBN / 4 + 2 * j + 1] = p2.y;
-        }
+        for (int rr = 0; rr < 2; ++rr) locate(rr, valid[rr], pix[rr], rpix[rr], spi[rr]);
+        auto loads_landed = [&] {
 #ifdef EMO_CONV_DEBUG
-        if (p.dbg & 512) {
-          // phase clocks: wait for the loads here, so that their latency is counted as load time
-          float s = 0.f;
+          if (p.dbg & 512) {
+            // phase clocks: wait for the loads here, so that their latency is counted as load time
+            float s = 0.f;
 #pragma unroll
-          for (int j = 0; j < kMaxBN / 2; ++j) s += cf[j];
-          if (s == 1.2345e-38f) g_conv_phase[0] = 0;
-        }
+            for (int j = 0; j < kMaxBN / 2; ++j) s += cf[j];
+            if (s == 1.2345e-38f) g_conv_phase[0] = 0;
+          }
 #endif
-        EMO_PHASE(2);
+          EMO_PHASE(2);
+        };
+        // act(v + residual), then the post-add as a separate rounding (__fadd_rn: never contracted into the activation's
+        // last multiply; + 0 without one), then the stores; zero outside the tensor, so that those pixels / channels are no
+        // part of the statistics
+        auto finish_row = [&](int rr, const float* res, const float* post) {
 #pragma unroll
-        for (int j = 0; j < kMaxBN / 8; ++j) {
-          if (8 * j >= BN) continue;
-          const int c = n0 + 8 * j + cq;
-          float v0 = acc[4 * j + 2 * rr], v1 = acc[4 * j + 2 * rr + 1];
-          if (valid && c < p.Cout && !EMO_DBG(8)) {
-            if constexpr (pairs) {
-              // __fadd_rn: the post-add stays a separate rounding (never contracted into the activation's last multiply)
-              v0 = __fadd_rn(act_apply(v0 + cf[2 * j], act), cf[kMaxBN / 4 + 2 * j]);
-              v1 = __fadd_rn(act_apply(v1 + cf[2 * j + 1], act), cf[kMaxBN / 4 + 2 * j + 1]);
+          for (int j = 0; j < kMaxBN / 8; ++j) {
+            if (8 * j >= BN) continue;
+            const int c = n0 + 8 * j + cq;
+            float v0 = 0.f, v1 = 0.f;
+            if (valid[rr] && c < p.Cout && !EMO_DBG(8)) {
+              v0 = __fadd_rn(act_apply(acc[4 * j + 2 * rr] + res[2 * j], act), post ? post[2 * j] : 0.f);
+              v1 = __fadd_rn(act_apply(acc[4 * j + 2 * rr + 1] + res[2 * j + 1], act), post ? post[2 * j + 1] : 0.f);
               if (!p.out_nchw) {
-                *(float2*)(p.out + pix * p.Cout + c) = make_float2(v0, v1);
+                *(float2*)(p.out + pix[rr] * p.Cout + c) = make_float2(v0, v1);
               } else {
-                p.out[((long long)n * p.Cout + c) * sp + spi] = v0;
-                p.out[((long long)n * p.Cout + c + 1) * sp + spi] = v1;
-              }
-            } else {
-              // odd channel count (e.g. Cout = 3): scalar path
-#pragma unroll
-              for (int q = 0; q < 2; ++q) {
-                const int cc = c + q;
-                float x = q ? v1 : v0;
-                if (cc < p.Cout) {
-                  if (p.residual) x += __ldg(p.residual + rpix * p.Cout + cc);
-                  x = act_apply(x, act);
-                  if (p.post_add) x += __ldg(p.post_add + spi * p.Cout + cc);
-                  if (!p.out_nchw) p.out[pix * p.Cout + cc] = x;
-                  else p.out[((long long)n * p.Cout + cc) * sp + spi] = x;
-                } else {
-                  x = 0.f;
-                }
-                if (q) v1 = x; else v0 = x;
+                p.out[((long long)n * p.Cout + c) * sp + spi[rr]] = v0;
+                p.out[((long long)n * p.Cout + c + 1) * sp + spi[rr]] = v1;
               }
             }
-          } else {
-            v0 = 0.f; v1 = 0.f;  // pixels / channels outside the tensor: no part of the statistics
+            acc[4 * j + 2 * rr] = v0; acc[4 * j + 2 * rr + 1] = v1;
           }
-          acc[4 * j + 2 * rr] = v0; acc[4 * j + 2 * rr + 1] = v1;
+        };
+        if (!p.post_add) {
+          load_pairs(cf, p.residual, rpix[0], valid[0]);
+          load_pairs(cf + kMaxBN / 4, p.residual, rpix[1], valid[1]);
+          loads_landed();
+          finish_row(0, cf, nullptr);
+          finish_row(1, cf + kMaxBN / 4, nullptr);
+        } else {
+#pragma unroll
+          for (int rr = 0; rr < 2; ++rr) {
+            load_pairs(cf, p.residual, rpix[rr], valid[rr]);
+            load_pairs(cf + kMaxBN / 4, p.post_add, spi[rr], valid[rr]);
+            loads_landed();
+            finish_row(rr, cf, cf + kMaxBN / 4);
+            EMO_PHASE(3);
+          }
         }
-        EMO_PHASE(3);
+        if (!p.post_add) EMO_PHASE(3);
+      } else {
+        // odd channel count (e.g. Cout = 3): scalar path
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr) {
+          bool valid;
+          long long pix, rpix, spi;
+          locate(rr, valid, pix, rpix, spi);
+          EMO_PHASE(2);
+#pragma unroll
+          for (int j = 0; j < kMaxBN / 8; ++j) {
+            if (8 * j >= BN) continue;
+            const int c = n0 + 8 * j + cq;
+#pragma unroll
+            for (int q = 0; q < 2; ++q) {
+              const int cc = c + q;
+              float x = acc[4 * j + 2 * rr + q];
+              if (valid && cc < p.Cout && !EMO_DBG(8)) {
+                if (p.residual) x += __ldg(p.residual + rpix * p.Cout + cc);
+                x = act_apply(x, act);
+                if (p.post_add) x += __ldg(p.post_add + spi * p.Cout + cc);
+                if (!p.out_nchw) p.out[pix * p.Cout + cc] = x;
+                else p.out[((long long)n * p.Cout + cc) * sp + spi] = x;
+              } else {
+                x = 0.f;  // pixels / channels outside the tensor: no part of the statistics
+              }
+              acc[4 * j + 2 * rr + q] = x;
+            }
+          }
+          EMO_PHASE(3);
+        }
       }
     };
     using std::integral_constant;
@@ -1192,7 +1238,9 @@ static int plan_conv(const emo_conv_desc* d, int sm_count, ConvPlan* plan) {
   }
   EMO_REQUIRE(plan->kernel >= 0, "emo_conv_igemm: internal error: no kernel for NP=%d fp16=%d upconv=%d KC=%d", NP, f16, ps, KC);
   plan->grid = grid;
-  plan->smem_bytes = smem_bytes;
+  // the per-CTA bias copy is placed after planning, above the planned area, where the opt-in maximum leaves room
+  p.bias_smem = (d->bias && ksplit == 1 && p.ntc == 1 && smem_bytes + kMaxBN * sizeof(float) <= smem_limit) ? 1 : 0;
+  plan->smem_bytes = smem_bytes + (p.bias_smem ? kMaxBN * sizeof(float) : 0);
   return EMO_OK;
 }
 
@@ -1247,6 +1295,7 @@ extern "C" int emo_conv_igemm(const emo_conv_desc* d, void* stream_) {
   const int NP = plan.NP, KC = plan.KC, f16 = plan.f16, ps = plan.ps, kh_eff = plan.kh_eff, BN = p.BN, ksplit = p.ksplit;
   const int grid = plan.grid;
   const size_t smem_bytes = plan.smem_bytes;
+  EMO_REQUIRE(smem_bytes <= 227 * 1024, "emo_conv_igemm: internal error: %zu bytes of shared memory", smem_bytes);
 
   // ---- tensor maps ----
   TMaps tm;
