@@ -126,6 +126,15 @@ __device__ __forceinline__ float warp_sum(float v) {
   return v;
 }
 
+// The video loop's foreground / background blend of one value (E_emo_infer_video.ipynb cell 41): m' = (m > thr ? m : 0)^8,
+// m' * *img + (1 - m') * *bg.  composite_kernel and the bilinear taps of s2_prepare_composite_kernel both call it, so they give
+// the same bits.
+__device__ __forceinline__ float composite_pixel(float m, const float* img, const float* bg, float thr) {
+  m = m > thr ? m : 0.f;
+  const float m2 = m * m, m4 = m2 * m2, m8 = m4 * m4;
+  return m8 * __ldg(img) + (1.f - m8) * __ldg(bg);
+}
+
 __device__ __forceinline__ float act_apply(float v, int act) {
   switch (act) {
     case EMO_ACT_RELU: return fmaxf(v, 0.f);

@@ -450,11 +450,31 @@ struct ResizeParams {
   float* out;
 };
 
+// A bilinear_pixel source that reads composite_pixel(matte, img, bg) (composite_kernel's output, never written to memory) in
+// place of an image value: image n of img (N,C,H,W) and matte (N,1,H,W), over bg (C,H,W).  bilinear_pixel offsets it by the
+// channel plane (the matte has one plane) and then by the pixel, as it offsets a plain NCHW pointer.
+struct CompositeAt {
+  const float *img, *matte, *bg;
+  float thr;
+  __device__ __forceinline__ CompositeAt operator+(int i) const { return CompositeAt{img + i, matte + i, bg + i, thr}; }
+};
+struct CompositeSrc {
+  const float *img, *matte, *bg;
+  float thr;
+  __device__ __forceinline__ CompositeSrc(const float* img, const float* matte, const float* bg, float thr, int n, int C, long long HW)
+      : img(img + (long long)n * C * HW), matte(matte + n * HW), bg(bg), thr(thr) {}
+  __device__ __forceinline__ CompositeAt operator+(long long plane) const { return CompositeAt{img + plane, matte, bg + plane, thr}; }
+};
+// bilinear_pixel's taps read __ldg(plane + offset); this overload makes that the composited value
+using ::__ldg;
+__device__ __forceinline__ float __ldg(const CompositeAt& p) { return composite_pixel(__ldg(p.matte), p.img, p.bg, p.thr); }
+
 // One output pixel (n, oh, ow) of the bilinear resize, sh = Hin / Hout, sw = Win / Wout: for every channel c < C_pad,
-// emit(c, v) with v = post(c, interpolation of input channel c) for c < C and v = 0 above.  resize_bilinear_kernel and
-// s2_prepare_kernel both call it, so the stage-2 input is the same bits as emo_resize_bilinear's.
-template <class Post, class Emit>
-__device__ __forceinline__ void bilinear_pixel(const float* in, int n, int C, int C_pad, int Hin, int Win, int oh, int ow, float sh,
+// emit(c, v) with v = post(c, interpolation of input channel c) for c < C and v = 0 above.  resize_bilinear_kernel,
+// s2_prepare_kernel and s2_prepare_composite_kernel all call it, so the stage-2 input is the same bits as emo_resize_bilinear's
+// of the same input values.
+template <class Src, class Post, class Emit>
+__device__ __forceinline__ void bilinear_pixel(Src in, int n, int C, int C_pad, int Hin, int Win, int oh, int ow, float sh,
                                                float sw, Post post, Emit emit) {
   float sy = fmaxf(((float)oh + 0.5f) * sh - 0.5f, 0.f);
   float sx = fmaxf(((float)ow + 0.5f) * sw - 0.5f, 0.f);
@@ -465,7 +485,7 @@ __device__ __forceinline__ void bilinear_pixel(const float* in, int n, int C, in
   for (int c = 0; c < C_pad; ++c) {
     float acc = 0.f;
     if (c < C) {
-      const float* s = in + ((long long)n * C + c) * Hin * Win;
+      const auto s = in + ((long long)n * C + c) * Hin * Win;
       acc = hy * (hx * __ldg(s + y0 * Win + x0) + lx * __ldg(s + y0 * Win + x1)) +
             ly * (hx * __ldg(s + y1 * Win + x0) + lx * __ldg(s + y1 * Win + x1));
       acc = post(c, acc);
@@ -492,32 +512,25 @@ __global__ void resize_bilinear_kernel(const ResizeParams p) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// the stage-1 -> stage-2 handoff of a refined frame (emo_s2_prepare, emo_s2_finish)
+// the stage-1 -> stage-2 handoff of a refined frame (emo_s2_prepare, emo_s2_prepare_composite, emo_s2_masked_stem,
+// emo_s2_finish, emo_s2_finish_masked)
 // ------------------------------------------------------------------------------------------------
-// One CTA = kS2Tile consecutive output pixels of one row of one image.  Each pixel's bilinear value is computed once by
-// bilinear_pixel and written as the NCHW `resized` image and as the stem's operand: the channels-last (R, G, B, 0) pixel of
-// emo_resize_bilinear (C_pad 4), or (FP16) the 7 horizontal taps of emo_stem_pack's plane, packed by plane4_h from the tile's
-// values and a 3-pixel halo on each side, staged in shared memory.
+// One CTA = kS2Tile consecutive output pixels of one row of one image.  Each pixel's value (R, G, B, 0) is computed once and
+// written by `out` (the NCHW `resized` image of the prepare passes) and as the stem's operand: the channels-last pixel itself
+// (kStemX4, emo_resize_bilinear's layout with C_pad 4), or the 7 horizontal taps of emo_stem_pack's plane (kStemPlane),
+// packed by plane4_h from the tile's values and a 3-pixel halo on each side, staged in shared memory; or no operand
+// (kStemNone).
 constexpr int kS2Tile = 256;
+enum { kStemNone = 0, kStemX4 = 1, kStemPlane = 2 };
 
-template <bool FP16>
-__global__ void __launch_bounds__(kS2Tile) s2_prepare_kernel(const float* __restrict__ img, int Hin, int Win, int S, float sh, float sw,
-                                                              float* __restrict__ resized, float4* __restrict__ x4, uint4* __restrict__ plane,
-                                                              float scale) {
-  __shared__ float4 row[kS2Tile + 6];
-  const int tiles = (S + kS2Tile - 1) / kS2Tile;
-  const int w0 = (int)(blockIdx.x % tiles) * kS2Tile;
-  const int oh = (int)((blockIdx.x / tiles) % S);
-  const int n = (int)(blockIdx.x / ((long long)tiles * S));
-  const auto pixel = [&](int ow) {
-    float v[4];
-    bilinear_pixel(img, n, 3, 4, Hin, Win, oh, ow, sh, sw, [](int, float acc) { return acc; }, [&](int c, float acc) { v[c] = acc; });
-    return make_float4(v[0], v[1], v[2], v[3]);
-  };
+// The tile [w0, w0 + kS2Tile) of output row oh of image n: out(ow, pixel(ow)) and the stem's operand of the pixels.
+template <int STEM, class Pixel, class Out>
+__device__ __forceinline__ void s2_tile(int n, int oh, int w0, int S, Pixel pixel, Out out, float4* __restrict__ x4, uint4* __restrict__ plane,
+                                        float scale, float4* row) {
   const int ow = w0 + (int)threadIdx.x;
   const long long HW = (long long)S * S;
   const long long pix = (long long)n * HW + (long long)oh * S + ow;
-  if (FP16) {
+  if (STEM == kStemPlane) {
     for (int i = threadIdx.x; i < kS2Tile + 6; i += kS2Tile) {
       const int x = w0 + i - 3;
       row[i] = (x >= 0 && x < S) ? pixel(x) : make_float4(0.f, 0.f, 0.f, 0.f);
@@ -525,9 +538,7 @@ __global__ void __launch_bounds__(kS2Tile) s2_prepare_kernel(const float* __rest
     __syncthreads();
     if (ow >= S) return;
     const float4 v = row[threadIdx.x + 3];
-    resized[(n * 3 + 0) * HW + (long long)oh * S + ow] = v.x;
-    resized[(n * 3 + 1) * HW + (long long)oh * S + ow] = v.y;
-    resized[(n * 3 + 2) * HW + (long long)oh * S + ow] = v.z;
+    out(ow, v);
     uint2 t[8];
 #pragma unroll
     for (int kx = 0; kx < 7; ++kx) {
@@ -541,15 +552,90 @@ __global__ void __launch_bounds__(kS2Tile) s2_prepare_kernel(const float* __rest
   } else {
     if (ow >= S) return;
     const float4 v = pixel(ow);
-    resized[(n * 3 + 0) * HW + (long long)oh * S + ow] = v.x;
-    resized[(n * 3 + 1) * HW + (long long)oh * S + ow] = v.y;
-    resized[(n * 3 + 2) * HW + (long long)oh * S + ow] = v.z;
-    x4[pix] = v;
+    out(ow, v);
+    if (STEM == kStemX4) x4[pix] = v;
   }
 }
 
-// ffhq = clamp(resized + add, 0, 1) as torch computes it (one fp32 add, NaN kept), and its uint8 frame as image_to_u8_kernel
-// writes it (trunc(clamp(x, 0, 1) * 255), NaN -> 0): thread = one pixel of the 3-channel NCHW images.
+// The prepare passes: pixel(n, oh, ow) is the bilinear resize of image n of the stage-1 image (plain, or composited), written to
+// the NCHW `resized` image (N,3,S,S) and as the stem's operand.
+template <int STEM, class Pixel>
+__device__ __forceinline__ void s2_prepare_tile(int S, Pixel pixel_of, float* __restrict__ resized, float4* __restrict__ x4,
+                                                uint4* __restrict__ plane, float scale, float4* row) {
+  const int tiles = (S + kS2Tile - 1) / kS2Tile;
+  const int w0 = (int)(blockIdx.x % tiles) * kS2Tile;
+  const int oh = (int)((blockIdx.x / tiles) % S);
+  const int n = (int)(blockIdx.x / ((long long)tiles * S));
+  const auto pixel = [&](int ow) { return pixel_of(n, oh, ow); };
+  const long long HW = (long long)S * S;
+  const auto out = [&](int ow, const float4& v) {
+    resized[(n * 3 + 0) * HW + (long long)oh * S + ow] = v.x;
+    resized[(n * 3 + 1) * HW + (long long)oh * S + ow] = v.y;
+    resized[(n * 3 + 2) * HW + (long long)oh * S + ow] = v.z;
+  };
+  s2_tile<STEM>(n, oh, w0, S, pixel, out, x4, plane, scale, row);
+}
+
+template <bool FP16>
+__global__ void __launch_bounds__(kS2Tile) s2_prepare_kernel(const float* __restrict__ img, int Hin, int Win, int S, float sh, float sw,
+                                                              float* __restrict__ resized, float4* __restrict__ x4, uint4* __restrict__ plane,
+                                                              float scale) {
+  __shared__ float4 row[kS2Tile + 6];
+  const auto pixel = [&](int n, int oh, int ow) {
+    float v[4];
+    bilinear_pixel(img, n, 3, 4, Hin, Win, oh, ow, sh, sw, [](int, float acc) { return acc; }, [&](int c, float acc) { v[c] = acc; });
+    return make_float4(v[0], v[1], v[2], v[3]);
+  };
+  s2_prepare_tile<FP16 ? kStemPlane : kStemX4>(S, pixel, resized, x4, plane, scale, row);
+}
+
+// s2_prepare_kernel of the composited image: every bilinear tap reads composite_pixel(matte, img, bg) (composite_kernel's value)
+// in place of the stage-1 pixel.  matte (N,1,Hin,Win), bg (3,Hin,Win).
+template <int STEM>
+__global__ void __launch_bounds__(kS2Tile) s2_prepare_composite_kernel(const float* __restrict__ img, const float* __restrict__ matte,
+                                                                        const float* __restrict__ bg, float thr, int Hin, int Win, int S,
+                                                                        float sh, float sw, float* __restrict__ resized,
+                                                                        float4* __restrict__ x4, uint4* __restrict__ plane, float scale) {
+  __shared__ float4 row[kS2Tile + 6];
+  const auto pixel = [&](int n, int oh, int ow) {
+    float v[4];
+    bilinear_pixel(CompositeSrc(img, matte, bg, thr, n, 3, (long long)Hin * Win), 0, 3, 4, Hin, Win, oh, ow, sh, sw,
+                   [](int, float acc) { return acc; }, [&](int c, float acc) { v[c] = acc; });
+    return make_float4(v[0], v[1], v[2], v[3]);
+  };
+  s2_prepare_tile<STEM>(S, pixel, resized, x4, plane, scale, row);
+}
+
+// The stem's operand of resized * matte (torch's x4 * mask of Stage2Model.forward: (R m, G m, B m, 0 m), one fp32 product each).
+// resized (N,3,S,S), matte (N,1,S,S).
+template <int STEM>
+__global__ void __launch_bounds__(kS2Tile) s2_masked_stem_kernel(const float* __restrict__ resized, const float* __restrict__ matte, int S,
+                                                                  float4* __restrict__ x4, uint4* __restrict__ plane, float scale) {
+  __shared__ float4 row[kS2Tile + 6];
+  const int tiles = (S + kS2Tile - 1) / kS2Tile;
+  const int w0 = (int)(blockIdx.x % tiles) * kS2Tile;
+  const int oh = (int)((blockIdx.x / tiles) % S);
+  const int n = (int)(blockIdx.x / ((long long)tiles * S));
+  const long long HW = (long long)S * S;
+  const auto pixel = [&](int ow) {
+    const long long s = (long long)oh * S + ow;
+    const float m = __ldg(matte + n * HW + s);
+    return make_float4(__fmul_rn(__ldg(resized + (n * 3 + 0) * HW + s), m), __fmul_rn(__ldg(resized + (n * 3 + 1) * HW + s), m),
+                       __fmul_rn(__ldg(resized + (n * 3 + 2) * HW + s), m), __fmul_rn(0.f, m));
+  };
+  s2_tile<STEM>(n, oh, w0, S, pixel, [](int, const float4&) {}, x4, plane, scale, row);
+}
+
+// ffhq = clamp(x, 0, 1) as torch's clamp_ computes it (a NaN stays NaN) into out[i], and its uint8 value as image_to_u8_kernel
+// writes it (trunc(clamp(x, 0, 1) * 255), NaN -> 0) into u8[o]
+__device__ __forceinline__ void s2_store(float x, long long i, long long o, float* __restrict__ out, unsigned char* __restrict__ u8) {
+  const float y = x != x ? x : fminf(fmaxf(x, 0.f), 1.f);
+  out[i] = y;
+  const float v = fminf(fmaxf(y, 0.f), 1.f) * 255.f;
+  u8[o] = (unsigned char)(int)v;
+}
+
+// ffhq = clamp(resized + add, 0, 1) (one fp32 add) and its uint8 frame: thread = one pixel of the 3-channel NCHW images.
 __global__ void __launch_bounds__(256) s2_finish_kernel(const float* __restrict__ resized, const float* __restrict__ add, int N, long long HW,
                                                         float* __restrict__ out, unsigned char* __restrict__ u8) {
   const long long total = (long long)N * HW;
@@ -558,11 +644,25 @@ __global__ void __launch_bounds__(256) s2_finish_kernel(const float* __restrict_
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
       const long long i = (n * 3 + c) * HW + s;
-      const float x = __fadd_rn(__ldg(resized + i), __ldg(add + i));
-      const float y = x != x ? x : fminf(fmaxf(x, 0.f), 1.f);
-      out[i] = y;
-      const float v = fminf(fmaxf(y, 0.f), 1.f) * 255.f;
-      u8[t * 3 + c] = (unsigned char)(int)v;
+      s2_store(__fadd_rn(__ldg(resized + i), __ldg(add + i)), i, t * 3 + c, out, u8);
+    }
+  }
+}
+
+// s2_finish_kernel with the residual mask of Stage2Model.forward: clamp(resized + add * (matte * face), 0, 1) as torch computes
+// it (fm = matte * face, add * fm, resized + add: one rounding each), face (N,1,H,W) uint8 0 / 1 or null (fm = matte).
+__global__ void __launch_bounds__(256) s2_finish_masked_kernel(const float* __restrict__ resized, const float* __restrict__ add,
+                                                               const float* __restrict__ matte, const unsigned char* __restrict__ face, int N,
+                                                               long long HW, float* __restrict__ out, unsigned char* __restrict__ u8) {
+  const long long total = (long long)N * HW;
+  for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (long long)gridDim.x * blockDim.x) {
+    const long long n = t / HW, s = t - n * HW;
+    const float m = __ldg(matte + t);
+    const float fm = face ? __fmul_rn(m, (float)face[t]) : m;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      const long long i = (n * 3 + c) * HW + s;
+      s2_store(__fadd_rn(__ldg(resized + i), __fmul_rn(__ldg(add + i), fm)), i, t * 3 + c, out, u8);
     }
   }
 }
@@ -827,4 +927,64 @@ extern "C" int emo_s2_finish(const float* resized, const float* add, int N, int 
   if (blocks > 132ll * 16) blocks = 132ll * 16;
   launch_kernel(s2_finish_kernel, (unsigned)blocks, 256, 0, stream, resized, add, N, (long long)H * W, out, u8);
   return check_launch("emo_s2_finish");
+}
+
+static bool f32_aligned(const void* p) { return ((uintptr_t)p % 4) == 0; }
+
+extern "C" int emo_s2_prepare_composite(const float* img, const float* matte, const float* bg, float threshold, int N, int Hin, int Win,
+                                        int S, float* resized, float* x4, void* plane, float plane_scale, void* stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  EMO_REQUIRE(img && matte && bg && resized, "emo_s2_prepare_composite: null pointer");
+  EMO_REQUIRE(!(x4 && plane), "emo_s2_prepare_composite: at most one stem operand (x4 or plane) may be given");
+  EMO_REQUIRE(N > 0 && Hin > 0 && Win > 0 && S > 0, "emo_s2_prepare_composite: bad shape (N=%d Hin=%d Win=%d S=%d)", N, Hin, Win, S);
+  EMO_REQUIRE(f32_aligned(img) && f32_aligned(matte) && f32_aligned(bg) && f32_aligned(resized),
+              "emo_s2_prepare_composite: fp32 tensors must be 4-byte aligned");
+  if (x4 || plane)
+    EMO_REQUIRE(((uintptr_t)(x4 ? (const void*)x4 : plane) % 16) == 0, "emo_s2_prepare_composite: the stem operand must be 16-byte aligned");
+  if (plane) EMO_REQUIRE(plane_scale > 0.f, "emo_s2_prepare_composite: plane_scale must be positive");
+  const long long blocks = (long long)N * S * cdiv(S, kS2Tile);
+  EMO_REQUIRE(blocks < (1ll << 31), "emo_s2_prepare_composite: grid too large");
+  const float sh = (float)Hin / (float)S, sw = (float)Win / (float)S;
+  const auto go = [&](auto kernel) {
+    launch_kernel(kernel, (unsigned)blocks, kS2Tile, 0, stream, img, matte, bg, threshold, Hin, Win, S, sh, sw, resized, (float4*)x4,
+                  (uint4*)plane, plane ? plane_scale : 0.f);
+  };
+  if (plane) go(s2_prepare_composite_kernel<kStemPlane>);
+  else if (x4) go(s2_prepare_composite_kernel<kStemX4>);
+  else go(s2_prepare_composite_kernel<kStemNone>);
+  return check_launch("emo_s2_prepare_composite");
+}
+
+extern "C" int emo_s2_masked_stem(const float* resized, const float* matte, int N, int S, float* x4, void* plane, float plane_scale,
+                                  void* stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  EMO_REQUIRE(resized && matte, "emo_s2_masked_stem: null pointer");
+  EMO_REQUIRE((x4 != nullptr) != (plane != nullptr), "emo_s2_masked_stem: exactly one stem operand (x4 or plane) must be given");
+  EMO_REQUIRE(N > 0 && S > 0, "emo_s2_masked_stem: bad shape (N=%d S=%d)", N, S);
+  EMO_REQUIRE(f32_aligned(resized) && f32_aligned(matte), "emo_s2_masked_stem: fp32 tensors must be 4-byte aligned");
+  EMO_REQUIRE(((uintptr_t)(x4 ? (const void*)x4 : plane) % 16) == 0, "emo_s2_masked_stem: the stem operand must be 16-byte aligned");
+  if (plane) EMO_REQUIRE(plane_scale > 0.f, "emo_s2_masked_stem: plane_scale must be positive");
+  const long long blocks = (long long)N * S * cdiv(S, kS2Tile);
+  EMO_REQUIRE(blocks < (1ll << 31), "emo_s2_masked_stem: grid too large");
+  if (plane)
+    launch_kernel(s2_masked_stem_kernel<kStemPlane>, (unsigned)blocks, kS2Tile, 0, stream, resized, matte, S, (float4*)nullptr,
+                  (uint4*)plane, plane_scale);
+  else
+    launch_kernel(s2_masked_stem_kernel<kStemX4>, (unsigned)blocks, kS2Tile, 0, stream, resized, matte, S, (float4*)x4, (uint4*)nullptr,
+                  0.f);
+  return check_launch("emo_s2_masked_stem");
+}
+
+extern "C" int emo_s2_finish_masked(const float* resized, const float* add, const float* matte, const unsigned char* face, int N, int H,
+                                    int W, float* out, unsigned char* u8, void* stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  EMO_REQUIRE(resized && add && matte && out && u8, "emo_s2_finish_masked: null pointer");
+  EMO_REQUIRE(N > 0 && H > 0 && W > 0, "emo_s2_finish_masked: bad shape (N=%d H=%d W=%d)", N, H, W);
+  EMO_REQUIRE(f32_aligned(resized) && f32_aligned(add) && f32_aligned(matte) && f32_aligned(out),
+              "emo_s2_finish_masked: fp32 tensors must be 4-byte aligned");
+  const long long total = (long long)N * H * W;
+  long long blocks = cdivll(total, 256);
+  if (blocks > 132ll * 16) blocks = 132ll * 16;
+  launch_kernel(s2_finish_masked_kernel, (unsigned)blocks, 256, 0, stream, resized, add, matte, face, N, (long long)H * W, out, u8);
+  return check_launch("emo_s2_finish_masked");
 }

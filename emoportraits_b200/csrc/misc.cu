@@ -357,10 +357,7 @@ __global__ void __launch_bounds__(256) composite_kernel(const float* __restrict_
     const long long nc = t / HW;
     const int c = (int)(nc % C);
     const long long n = nc / C;
-    float m = __ldg(mask + n * HW + s);
-    m = m > thr ? m : 0.f;
-    const float m2 = m * m, m4 = m2 * m2, m8 = m4 * m4;
-    out[t] = m8 * __ldg(img + t) + (1.f - m8) * __ldg(bg + (long long)c * HW + s);
+    out[t] = composite_pixel(__ldg(mask + n * HW + s), img + t, bg + (long long)c * HW + s, thr);
   }
 }
 
@@ -379,7 +376,7 @@ extern "C" int emo_composite(const float* img, const float* mask, const float* b
 }
 
 extern "C" const char* emo_last_error(void) { return emo::g_err; }
-extern "C" int emo_version(void) { return 108; }  // 101: emo_pose_desc (+theta_in, mix_old, smoothing) and emo_conv_desc (+upconv) grew trailing fields
+extern "C" int emo_version(void) { return 109; }  // 101: emo_pose_desc (+theta_in, mix_old, smoothing) and emo_conv_desc (+upconv) grew trailing fields
 
 extern "C" int emo_device_info(int* sm_count, int* cc) {
   int dev = 0;

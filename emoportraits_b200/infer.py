@@ -13,6 +13,7 @@ stubbed reference oracle uses too) and `modnet_mask=True` raises.
 """
 from __future__ import annotations
 
+import copy
 import pathlib
 from collections import OrderedDict
 from types import SimpleNamespace
@@ -216,9 +217,31 @@ class Model:
             raise ValueError(f"the stage-2 model is on {refine.device}, the stage-1 model on {self.device}: refined frames run "
                              "both on one device")
 
+    @staticmethod
+    def check_refine_masks(refine, refine_masks: Optional[dict] = None, composite=None) -> None:
+        """ValueError unless stage 2's mask networks refine_masks (dict(modnet=, face_idt=, cloth=), Stage2Model.refine) and the
+        compositing matte network `composite` can run in a refined frame of `refine`"""
+        if refine is None:
+            if refine_masks or composite is not None:
+                raise ValueError("refine_masks= and composite= act on stage 2: they need refine=")
+            return
+        if composite is not None and not callable(composite):
+            raise ValueError(f"composite must be a callable img (1,3,H,W) -> matte (1,1,H,W), got {type(composite).__name__}")
+        rm = dict(refine_masks or {})
+        if set(rm) - {"modnet", "face_idt", "cloth"}:
+            raise ValueError(f"refine_masks takes modnet, face_idt and cloth, got {sorted(rm)}")
+        if rm.get("modnet") is not None and not callable(rm["modnet"]):
+            raise ValueError(f"refine_masks['modnet'] must be the matting network (a callable), got {type(rm['modnet']).__name__}")
+        if rm.get("face_idt") is not None:
+            if rm.get("modnet") is None:
+                raise ValueError("stage 2's face mask multiplies the MODNet matte: refine_masks needs modnet with face_idt")
+            if not callable(getattr(rm["face_idt"], "label_masks", None)):
+                raise ValueError("refine_masks['face_idt'] must be a masks.FaceParsing: a captured frame keeps its uint8 label masks")
+
     def make_driver_graph(self, st, mix: bool = True, target_theta: bool = True, slot: int = 0, mix_old: bool = False,
                           smooth_state: Optional[torch.Tensor] = None, smooth_momentum: float = 0.5, image: bool = True,
-                          theta_embed: bool = False, pose_embed: bool = False, encode: bool = False, refine=None):
+                          theta_embed: bool = False, pose_embed: bool = False, encode: bool = False, refine=None,
+                          refine_masks: Optional[dict] = None, composite=None):
         """Capture one driver frame (all ~240 kernel launches) into a CUDA graph: removes the Python/ctypes launch
         overhead from the per-frame loop.  Returns replay(drv (1,3,H,W) on device) -> img (1,3,H,W) (static buffer).
         The graph reads its identity from buffers of its own (replay.identity, dist.new_identity), never from `st`:
@@ -238,18 +261,26 @@ class Model:
         refine (a stage2.Stage2Model on this device): the graph continues with stage 2 on the frame's image
         (Stage2Model.refine, the stage-2 wrapper's default masks): replay.static_out is then the refined (1,3,S2,S2) image,
         replay.static_u8 its (1,S2,S2,3) uint8 frame and replay.static_stage1 the stage-1 image.  The warm-up passes run
-        stage 2 under the same scratch set, so its workspaces exist before the capture."""
+        stage 2 under the same scratch set, so its workspaces exist before the capture.
+        refine_masks (dict(modnet=, face_idt=, cloth=), with refine): stage 2 runs with the masks these networks give
+        (Stage2Model.refine), the stage-2 wrapper's masks when they are plugged into it.  composite (a callable img (1,3,H,W) ->
+        matte (1,1,H,W), with refine, e.g. masks.face_matte): the stage-1 image is composited over replay.static_bg (3,H,W),
+        which the caller fills before a replay, as video.connect_img_and_bg does, before stage 2.  The caller's networks are
+        captured with the frame (INTEGRATION.md "Mask networks in captured frames": no host syncs, static shapes, already on
+        this device); the warm-up passes run them too.  A capture that fails raises RuntimeError naming the network that
+        broke it."""
         self.check_inputs(image, theta_embed, pose_embed, encode)
         self.check_refine(refine, encode)
+        self.check_refine_masks(refine, refine_masks, composite)
         prev = ops.set_slot(slot)
         try:
             return self._make_driver_graph(st, mix, target_theta, mix_old, smooth_state, smooth_momentum, image, theta_embed,
-                                           pose_embed, encode, refine)
+                                           pose_embed, encode, refine, refine_masks, composite)
         finally:
             ops.set_slot(prev)
 
     def _make_driver_graph(self, st, mix, target_theta, mix_old=False, smooth_state=None, smooth_momentum=0.5, image=True,
-                           theta_embed=False, pose_embed=False, encode=False, refine=None):
+                           theta_embed=False, pose_embed=False, encode=False, refine=None, refine_masks=None, composite=None):
         s, dev = self.cfg.image_size, self.device
         static_in = torch.zeros((1, 3, s, s), dtype=torch.float32, device=dev) if image else None
         # the warm-up passes run on the unit pose (scale 1, no rotation or translation) and a zero embedding
@@ -289,30 +320,74 @@ class Model:
 
         replay.load, replay.identity = load, identity
         load(st)  # the warm-up and capture passes run on a real identity
+        static_bg = torch.zeros((3, s, s), dtype=torch.float32, device=dev) if composite is not None else None
+        culprit = []   # the caller's network that raised, if one did
+        refine_kw = _named_networks(dict(refine_masks or {}), composite, culprit)
+
+        def refined(img):
+            if refine_kw.get("composite") is not None:
+                matte = refine_kw["composite"](img)
+                if not isinstance(matte, torch.Tensor) or tuple(matte.shape) != (1, 1, s, s):
+                    got = tuple(matte.shape) if isinstance(matte, torch.Tensor) else type(matte).__name__
+                    raise ValueError(f"composite must return the matte (1,1,{s},{s}), got {got}")
+                return refine.refine(img, matte=matte, bg=static_bg, **{k: v for k, v in refine_kw.items() if k != "composite"})
+            return refine.refine(img, **refine_kw)
+
         side = torch.cuda.Stream(device=self.device)
         side.wait_stream(torch.cuda.current_stream(self.device))
-        with torch.cuda.stream(side):
-            for _ in range(2):
-                img = self.driver_pass(identity, static_in, **kw)[0]
+        try:
+            with torch.cuda.stream(side):
+                for _ in range(2):
+                    img = self.driver_pass(identity, static_in, **kw)[0]
+                    if refine is not None:
+                        refined(img)
+            torch.cuda.current_stream(self.device).wait_stream(side)
+            torch.cuda.synchronize(self.device)
+            graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(graph):
+                out = self.driver_pass(identity, static_in, **kw)
+                static_out = static_stage1 = out[0]
+                static_u8 = None
                 if refine is not None:
-                    refine.refine(img)
-        torch.cuda.current_stream(self.device).wait_stream(side)
-        torch.cuda.synchronize(self.device)
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph):
-            out = self.driver_pass(identity, static_in, **kw)
-            static_out = static_stage1 = out[0]
-            static_u8 = None
-            if refine is not None:
-                _, static_out, static_u8 = refine.refine(static_stage1)
+                    _, static_out, static_u8 = refined(static_stage1)
+        except Exception as e:
+            if not culprit:
+                raise
+            raise RuntimeError(f"the refined driver frame could not be captured: {culprit[0]} raised {type(e).__name__}: {e}.  "
+                               "A network in a captured frame must issue no host syncs, keep its shapes static and already be "
+                               "on this device (INTEGRATION.md \"Mask networks in captured frames\"); otherwise run stage 2 with "
+                               "its masks eagerly, with stage2.InferenceWrapper.forward") from e
         if smooth_state is not None:
             smooth_state.copy_(saved)
 
         replay.graph = graph
         replay.static_in, replay.static_out, replay.static_state = static_in, static_out, out[3]
         replay.static_theta, replay.static_pose = static_theta, static_pose
-        replay.static_stage1, replay.static_u8 = static_stage1, static_u8
+        replay.static_stage1, replay.static_u8, replay.static_bg = static_stage1, static_u8, static_bg
         return replay
+
+
+def _named_networks(refine_masks: dict, composite, culprit: list) -> dict:
+    """Stage2Model.refine's mask arguments, plus `composite`, with every caller network wrapped so that an exception it raises
+    first appends the network's name to `culprit` (make_driver_graph's capture error names it)"""
+    def named(fn, name):
+        def call(*a, **k):
+            try:
+                return fn(*a, **k)
+            except Exception:
+                culprit.append(name)
+                raise
+        return call
+
+    out = dict(refine_masks)
+    if out.get("modnet") is not None:
+        out["modnet"] = named(out["modnet"], "the stage-2 matting network (modnet)")
+    if out.get("face_idt") is not None:
+        out["face_idt"] = copy.copy(out["face_idt"])
+        out["face_idt"].net = named(out["face_idt"].net, "the stage-2 face parser (face_idt.net)")
+    if composite is not None:
+        out["composite"] = named(composite, "the compositing matte network (composite / mask_fn)")
+    return out
 
 
 class DriverPipeline:
@@ -335,22 +410,27 @@ class DriverPipeline:
 
     refine (a stage2.Stage2Model): every frame is refined by stage 2 in the same graph (Model.make_driver_graph):
     slot.run.static_out is the refined (1,3,S2,S2) image, slot.run.static_u8 its uint8 frame and slot.run.static_stage1 the
-    stage-1 image.  submit(..., u8_out=) copies the uint8 frame out on the frame's stream."""
+    stage-1 image.  submit(..., u8_out=) copies the uint8 frame out on the frame's stream.
+    refine_masks / composite: stage 2's mask networks and the compositing matte network (Model.make_driver_graph), captured
+    with every frame; a compositing pipeline's frames take submit(..., bg=)."""
 
     def __init__(self, model: "Model", st, depth: int = 2, mix: bool = True, target_theta: bool = True, mix_old: bool = False,
-                 image: bool = True, theta_embed: bool = False, pose_embed: bool = False, encode: bool = False, refine=None):
+                 image: bool = True, theta_embed: bool = False, pose_embed: bool = False, encode: bool = False, refine=None,
+                 refine_masks: Optional[dict] = None, composite=None):
         model.check_inputs(image, theta_embed, pose_embed, encode)
         model.check_refine(refine, encode)
+        Model.check_refine_masks(refine, refine_masks, composite)
         self.model, self.depth, self.n = model, depth, 0
         self.image, self.theta_embed, self.pose_embed, self.encode = image, theta_embed, pose_embed, encode
-        self.refine = refine
+        self.refine, self.composite = refine, composite
         self.st = st  # the current identity: frames submitted without st= animate it
         self.slots = []
         for k in self.scratch_slots(depth):
             run = model.make_driver_graph(st, mix=mix, target_theta=target_theta, slot=k, mix_old=mix_old, image=image,
-                                          theta_embed=theta_embed, pose_embed=pose_embed, encode=encode, refine=refine)
+                                          theta_embed=theta_embed, pose_embed=pose_embed, encode=encode, refine=refine,
+                                          refine_masks=refine_masks, composite=composite)
             self.slots.append(SimpleNamespace(run=run, stream=torch.cuda.Stream(device=model.device),
-                                              done=torch.cuda.Event(), busy=False))
+                                              done=torch.cuda.Event(), busy=False, bg=None))
 
     @staticmethod
     def scratch_slots(depth: int) -> list:
@@ -358,9 +438,17 @@ class DriverPipeline:
         (Model.source_pass / driver_pass on the current stream), which may overlap frames in flight."""
         return [k + 1 for k in range(depth)]
 
-    def _check_submit(self, drv, theta_embed, pose_embed, outs, u8_out=None) -> None:
-        """ValueError unless a frame's inputs are the ones the pipeline was captured for, of the right shapes, and u8_out
-        a (1,S2,S2,3) uint8 buffer of a refining pipeline"""
+    def _check_submit(self, drv, theta_embed, pose_embed, outs, u8_out=None, bg=None) -> None:
+        """ValueError unless a frame's inputs are the ones the pipeline was captured for, of the right shapes, u8_out
+        a (1,S2,S2,3) uint8 buffer of a refining pipeline and bg a (3,H,W) fp32 background of a compositing one"""
+        if (bg is not None) != (getattr(self, "composite", None) is not None):
+            raise ValueError("bg= is the background of a compositing pipeline (composite=): give it exactly when the pipeline "
+                             "composites")
+        if bg is not None:
+            s = self.model.cfg.image_size
+            if not isinstance(bg, torch.Tensor) or tuple(bg.shape) != (3, s, s) or bg.dtype != torch.float32:
+                got = (tuple(bg.shape), bg.dtype) if isinstance(bg, torch.Tensor) else type(bg).__name__
+                raise ValueError(f"bg must be a float32 tensor of shape {(3, s, s)}, got {got}")
         if u8_out is not None:
             if self.refine is None:
                 raise ValueError("u8_out: only a refining pipeline (refine=) writes a uint8 frame")
@@ -384,7 +472,7 @@ class DriverPipeline:
 
     def submit(self, drv: Optional[torch.Tensor], host_out: Optional[torch.Tensor] = None, dev_out: Optional[torch.Tensor] = None,
                st=None, theta_embed: Optional[torch.Tensor] = None, pose_embed: Optional[torch.Tensor] = None,
-               u8_out: Optional[torch.Tensor] = None):
+               u8_out: Optional[torch.Tensor] = None, bg: Optional[torch.Tensor] = None):
         """Queue one frame (device tensor, or pinned host tensor -> asynchronous H2D on the frame's stream).  If `host_out`
         (pinned) / `dev_out` is given the image is copied into it on the same stream.  Returns a ticket: ticket.done is an
         event recorded when this frame (and its copy-out) has finished (ticket.slot.done is the same event, i.e. always the
@@ -398,10 +486,13 @@ class DriverPipeline:
         them; they are copied into the slot's buffers on its stream like the image.  drv is None for an image-free
         pipeline.  Inputs other than the pipeline's, or of other shapes, raise ValueError before anything is queued.
         u8_out (1,S2,S2,3) uint8, pinned host or device (a refining pipeline only): the refined frame's uint8 image
-        (slot.run.static_u8) is copied into it on the frame's stream, before ticket.done."""
+        (slot.run.static_u8) is copied into it on the frame's stream, before ticket.done.
+        bg (3,H,W) fp32 (a compositing pipeline only, and then for every frame): the background the frame is composited over.  A
+        slot copies it into its buffer (slot.run.static_bg) on its stream only when it is a different tensor from the slot's
+        last one; the slot keeps a reference to it and marks it as in use by its stream, as replay.load does an identity."""
         if st is not None:
             check_identity(st, self.model.cfg)
-        self._check_submit(drv, theta_embed, pose_embed, (host_out, dev_out), u8_out)
+        self._check_submit(drv, theta_embed, pose_embed, (host_out, dev_out), u8_out, bg)
         if st is not None:
             self.st = st
         sl = self.slots[self.n % self.depth]
@@ -412,6 +503,11 @@ class DriverPipeline:
         sl.stream.wait_stream(torch.cuda.current_stream(self.model.device))
         with torch.cuda.stream(sl.stream), torch.no_grad():
             sl.run.load(self.st)
+            if bg is not None and bg is not sl.bg:
+                sl.run.static_bg.copy_(bg, non_blocking=True)
+                if bg.is_cuda:
+                    bg.record_stream(sl.stream)
+                sl.bg = bg
             for buf, t in inputs:
                 buf.copy_(t, non_blocking=True)
             sl.run.graph.replay()
@@ -548,17 +644,21 @@ class InferenceWrapper(torch.nn.Module):
     # while every slot holds ~4 GB (exact) of captured activations.  Two keep one frame's host-side work under the other's.
     REFINE_DEPTH = 2
 
-    def _driver_pipeline(self, mix, target_theta, mix_old, refine=None, **inputs):
+    def _driver_pipeline(self, mix, target_theta, mix_old, refine=None, refine_masks=None, composite=None, **inputs):
         """the captured four-in-flight pipeline of these options (DriverPipeline's image / theta_embed / pose_embed / encode,
-        and the stage-2 model that refines its frames, keyed with its precision); it serves every identity (submit(..., st=))"""
+        the stage-2 model that refines its frames, keyed with its precision, and the network objects of stage 2's masks and of
+        the composite, with cloth); it serves every identity (submit(..., st=))"""
         key = (bool(mix), bool(target_theta), bool(mix_old), tuple(sorted(inputs.items())))
         if refine is not None:
             key += (("refine", refine, refine.precision),)
+        if refine_masks or composite is not None:
+            rm = refine_masks or {}
+            key += (("masks", rm.get("modnet"), rm.get("face_idt"), bool(rm.get("cloth")), composite),)
         pipe = self._pipelines.pop(key, None)
         if pipe is None:
             depth = 4 if refine is None else self.REFINE_DEPTH
             pipe = DriverPipeline(self.model, self._state, depth=depth, mix=mix, target_theta=target_theta, mix_old=mix_old,
-                                  refine=refine, **inputs)
+                                  refine=refine, refine_masks=refine_masks, composite=composite, **inputs)
         self._pipelines[key] = pipe
         # the new pipeline's captures synchronized the device, so nothing of a dropped one is still running
         while len(self._pipelines) > self.PIPELINES:
@@ -693,24 +793,45 @@ class InferenceWrapper(torch.nn.Module):
 
     @torch.no_grad()
     def forward_refined(self, driver_images, inferer_s2, mix=False, target_theta=True, mix_old=True,
-                        custome_target_theta_embed=None, custome_target_pose_embed=None):
+                        custome_target_theta_embed=None, custome_target_pose_embed=None, bg=None, mask_fn=None):
         """Driver frames refined by stage 2, each in one captured graph: the stage-1 frame, then inferer_s2's stage 2
-        (a stage2.InferenceWrapper on this device, with its default masks) on its image, REFINE_DEPTH frames in flight.
-        The refining pipeline is cached with the others (PIPELINES), keyed by the stage-2 model and its precision.
+        (a stage2.InferenceWrapper on this device) on its image, REFINE_DEPTH frames in flight.  Stage 2 runs with the masks
+        of the networks plugged into inferer_s2 (modnet, face_idt, and its cloth setting), or unmasked without them.
+        bg (3,H,W) + mask_fn (img (1,3,H,W) -> (1,1,H,W), e.g. masks.face_matte): every stage-1 image is composited over bg
+        first, as video.connect_img_and_bg does.  The networks run inside the captured frames (INTEGRATION.md "Mask networks in
+        captured frames"); a capture they break raises RuntimeError before any frame is queued.
+        The refining pipeline is cached with the others (PIPELINES), keyed by the stage-2 model and its precision, the mask
+        network objects, cloth and mask_fn.
         driver_images: what forward's driver path takes (a list of PIL / numpy frames, converted as each is queued; a tensor
         batch; one image), with custome_target_theta_embed / custome_target_pose_embed as in forward (one pose / embedding
         for every frame).  driver_images=None with both embeddings: frames rendered from them as animate renders them,
         theta_embed (N,3) x 3 and pose_embed (N,E).  Returns (list[PIL] of the refined S2 x S2 frames, img (N,3,S2,S2) on
-        the device); frame i is inferer_s2.forward(self.forward(None, frame_i, ...)[1])[2][0].  Sets pred_target_theta,
+        the device); frame i is inferer_s2.forward(x)[2][0] with x = self.forward(None, frame_i, ...)[1], composited as
+        video.connect_img_and_bg(x, bg, mask_fn(x)) when bg and mask_fn are given.  Sets pred_target_theta,
         pred_target_srt and target_pose_embed of the last frame.  There is no smooth_pose form: smoothing is a recurrence
         over the frames, which this path does not run.  Refused before anything is queued: no source pass yet
-        (RuntimeError), a stage-2 wrapper on another device or inputs that do not fit (ValueError)."""
+        (RuntimeError), a stage-2 wrapper on another device, mask networks or inputs that do not fit (ValueError)."""
         if self._state is None:
             raise RuntimeError("forward_refined() called before a source image was given")
         s2 = getattr(inferer_s2, "model_two", None)
         if s2 is None:
             raise ValueError("inferer_s2 must be a stage2.InferenceWrapper")
+        if (bg is None) != (mask_fn is None):
+            raise ValueError("bg and mask_fn composite the frames together: give both, or neither")
+        extra = {}
+        modnet, face_idt = getattr(inferer_s2, "modnet", None), getattr(inferer_s2, "face_idt", None)
+        if modnet is not None or face_idt is not None:
+            extra["refine_masks"] = dict(modnet=modnet, face_idt=face_idt, cloth=bool(getattr(inferer_s2, "cloth", False)))
+        if mask_fn is not None:
+            extra["composite"] = mask_fn
+            s = self.cfg.image_size
+            bg = torch.as_tensor(bg)
+            if tuple(bg.shape) != (3, s, s) or not bg.is_floating_point():
+                raise ValueError(f"bg must be a floating-point background of shape {(3, s, s)}, got {tuple(bg.shape)} {bg.dtype}")
+            bg = bg.to(self.device, torch.float32).contiguous()
         self.model.check_refine(s2, encode=False)
+        Model.check_refine_masks(s2, extra.get("refine_masks"), mask_fn)
+        with_bg = (lambda kw: dict(kw, bg=bg)) if bg is not None else (lambda kw: kw)
         E = self.cfg.expr_channels
         if driver_images is None:
             if custome_target_theta_embed is None or custome_target_pose_embed is None:
@@ -721,8 +842,9 @@ class InferenceWrapper(torch.nn.Module):
             if pe.dim() != 2 or tuple(pe.shape) != (srt.shape[0], E):
                 raise ValueError(f"custome_target_pose_embed must be ({srt.shape[0]},{E}) (one row per pose), got {tuple(pe.shape)}")
             srt, pe = srt.to(self.device).contiguous(), pe.to(self.device).contiguous()
-            pipe = self._driver_pipeline(mix, target_theta, mix_old, refine=s2, image=False, theta_embed=True, pose_embed=True)
-            return self._render(pipe, srt.shape[0], lambda i: dict(drv=None, theta_embed=srt[i:i + 1], pose_embed=pe[i:i + 1]))
+            pipe = self._driver_pipeline(mix, target_theta, mix_old, refine=s2, **extra, image=False, theta_embed=True, pose_embed=True)
+            return self._render(pipe, srt.shape[0],
+                                lambda i: with_bg(dict(drv=None, theta_embed=srt[i:i + 1], pose_embed=pe[i:i + 1])))
         if isinstance(driver_images, list) and not driver_images:
             raise ValueError("forward_refined: no driver frame")
         srt = pe = None
@@ -738,8 +860,8 @@ class InferenceWrapper(torch.nn.Module):
                                  f"got {tuple(pe.shape)}")
             pe = pe.to(self.device).reshape(1, E).contiguous()
         n, frame = self._frames(driver_images)
-        pipe = self._driver_pipeline(mix, target_theta, mix_old, refine=s2, theta_embed=srt is not None, pose_embed=pe is not None)
-        return self._render(pipe, n, lambda i: dict(drv=frame(i), theta_embed=srt, pose_embed=pe))
+        pipe = self._driver_pipeline(mix, target_theta, mix_old, refine=s2, **extra, theta_embed=srt is not None, pose_embed=pe is not None)
+        return self._render(pipe, n, lambda i: with_bg(dict(drv=frame(i), theta_embed=srt, pose_embed=pe)))
 
     # -- notebooks/infer.py:229-243
     def convert_to_tensor(self, image):

@@ -141,6 +141,10 @@ SYMBOLS = {
     "emo_resize_bicubic": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "emo_s2_prepare": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_float, c_void_p]),
     "emo_s2_finish": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "emo_s2_prepare_composite": (c_int, [c_void_p, c_void_p, c_void_p, c_float, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
+                                         c_void_p, c_float, c_void_p]),
+    "emo_s2_masked_stem": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_float, c_void_p]),
+    "emo_s2_finish_masked": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "emo_composite": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p]),
     "emo_l2_flush": (c_int, [c_void_p, c_ll, c_void_p]),
     "emo_l2_flush_clean": (c_int, [c_void_p, c_ll, c_void_p]),

@@ -7,6 +7,7 @@ around them is here, with the network supplied by the caller (any callable with 
   FaceParsing            networks/volumetric_avatar/face_parcing.py:9-81 (same ctor arguments + `net=`; `forward` returns the same
                          four int64 masks)
   modnet_get_mask        notebooks/infer.py:649-684 (InferenceWrapper.get_mask)
+  face_matte             notebooks/E_emo_infer_video.ipynb cell 13 (get_mask_fp): the video loop's compositing matte
 
 Normalisation, both bilinear resizes, argmax, label-set membership and the two 'area' resizes are csrc/masks.cu kernels; the
 network in the middle runs as whatever the caller supplies (torch module on the same device)."""
@@ -55,13 +56,18 @@ class FaceParsing(object):
         self.mask_labels, self.face_labels, self.body_labels, self.cloth_labels = _LABELS_DEFAULT
 
     @torch.no_grad()
-    def forward(self, x):
-        """x (N,3,h,w) fp32 in [0,1] on the device -> (mask, face_body, mask_body, mask_cloth), int64 (N,1,h,w) like the reference."""
+    def label_masks(self, x):
+        """forward's four masks as one uint8 (4,N,1,h,w) tensor of 0 / 1, not widened to int64: what a captured frame keeps."""
         h, w = x.shape[2:]
         x512 = ops.parsing_prepare(x.to(self.device).float().contiguous(), self.mean, self.std, (512, 512))   # :57-58
         y = self.net(x512)[0]                                                                                # :59
         m = ops.parsing_masks(y.float().contiguous(), (h, w), (self.mask_labels, self.face_labels, self.body_labels, self.cloth_labels))
-        m = m.to(torch.int64)                                                                                # zeros_like(labels): int64
+        return m
+
+    @torch.no_grad()
+    def forward(self, x):
+        """x (N,3,h,w) fp32 in [0,1] on the device -> (mask, face_body, mask_body, mask_cloth), int64 (N,1,h,w) like the reference."""
+        m = self.label_masks(x).to(torch.int64)                                                              # zeros_like(labels): int64
         return m[0], m[1], m[2], m[3]
 
     __call__ = forward
@@ -88,3 +94,17 @@ def modnet_get_mask(modnet, img):
     im = ops.resize_area(img.float().contiguous(), (im_rh, im_rw), scale=2.0, shift=-1.0)
     _, _, matte = modnet(im, True)
     return ops.resize_area(matte.float().contiguous(), (im_h, im_w))
+
+
+def face_matte(face_idt, modnet):
+    """The video loop's compositing matte, E_emo_infer_video.ipynb cell 13 (get_mask_fp), as a callable img (N,3,h,w) ->
+    (N,1,h,w) fp32 usable as video.drive_image_with_video's / forward_refined's mask_fn: the face-parsing mask (> 0.6) times
+    the MODNet matte clamped to [0, 1].  face_idt: a FaceParsing; modnet: the matting network.  It issues no host sync, so a
+    captured frame may run it (INTEGRATION.md "Mask networks in captured frames")."""
+
+    @torch.no_grad()
+    def mask_fn(img):
+        face = (face_idt.forward(img)[0] > 0.6).float()
+        return face * modnet_get_mask(modnet, img).clamp_(max=1, min=0)
+
+    return mask_fn

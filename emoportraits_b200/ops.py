@@ -704,6 +704,68 @@ def s2_prepare(img_nchw: torch.Tensor, size: int, fast: bool):
     return resized, stem_in
 
 
+def _stem_operand(N: int, size: int, fast: bool, device):
+    """an empty stem operand of stage 2 at (N, size): (operand, x4, plane, scale) as the handoff entry points take them"""
+    if fast:
+        stem_in = Split.empty((N, 1, size, size, STEM_CIN), device, H1)
+        return stem_in, None, stem_in.hi, stem_in.scale
+    x4 = torch.empty((N, 1, size, size, 4), dtype=torch.float32, device=device)
+    return x4, x4, None, 0.0
+
+
+def s2_prepare_composite(img_nchw: torch.Tensor, matte: torch.Tensor, bg: torch.Tensor, size: int, fast: Optional[bool],
+                         threshold: float = 0.3):
+    """s2_prepare of composite(img, matte, bg, threshold) in one pass, the composited image never in memory: (resized, the stem's
+    operand, or None with fast=None, when the stem reads s2_masked_stem's operand instead).  img (N,3,h,w), matte (N,1,h,w),
+    bg (3,h,w) fp32.  Same bits as the two-step path."""
+    _chk(img_nchw); _chk(matte); _chk(bg)
+    N, Cc, Hi, Wi = img_nchw.shape
+    assert Cc == 3 and tuple(matte.shape) == (N, 1, Hi, Wi) and tuple(bg.shape) == (3, Hi, Wi), (img_nchw.shape, matte.shape, bg.shape)
+    resized = torch.empty((N, 3, size, size), dtype=torch.float32, device=img_nchw.device)
+    stem_in, x4, plane, scale = (None, None, None, 0.0) if fast is None else _stem_operand(N, size, fast, img_nchw.device)
+    L.call("emo_s2_prepare_composite", _p(img_nchw), _p(matte), _p(bg), C.c_float(threshold), N, Hi, Wi, size, _p(resized), _p(x4),
+           _p(plane), C.c_float(scale), _stream())
+    return resized, stem_in
+
+
+def s2_masked_stem(resized: torch.Tensor, matte: torch.Tensor, fast: bool, out=None):
+    """The stage-2 stem's operand of resized * matte (Stage2Model.forward's x4 * mask): resize_bilinear's (N,1,S,S,4) layout
+    (R m, G m, B m, 0 m), or with `fast` stem_pack() of it.  resized (N,3,S,S), matte (N,1,S,S) fp32.  out: an operand of
+    that kind to write in place.  Same bits as torch's product (then ops.stem_pack)."""
+    _chk(resized); _chk(matte)
+    N, Cc, S, S2 = resized.shape
+    assert Cc == 3 and S == S2 and tuple(matte.shape) == (N, 1, S, S), (resized.shape, matte.shape)
+    if out is None:
+        stem_in, x4, plane, scale = _stem_operand(N, S, fast, resized.device)
+    elif fast:
+        stem_in, x4, plane, scale = out, None, out.hi, out.scale
+    else:
+        stem_in, x4, plane, scale = out, out, None, 0.0
+    L.call("emo_s2_masked_stem", _p(resized), _p(matte), N, S, _p(x4), _p(plane), C.c_float(scale), _stream())
+    return stem_in
+
+
+def s2_finish_masked(resized: torch.Tensor, add: torch.Tensor, matte: torch.Tensor, face: Optional[torch.Tensor] = None,
+                     out: Optional[torch.Tensor] = None, u8: Optional[torch.Tensor] = None):
+    """(ffhq, u8): ffhq = (resized + add * (matte * face)).clamp_(0, 1) (N,3,H,W) fp32, Stage2Model.forward's masked residual,
+    and u8 = image_to_u8(ffhq), in one pass.  matte (N,1,H,W) fp32; face (N,1,H,W) uint8 0 / 1 (parsing_masks' first mask) or
+    None (cloth: matte alone)."""
+    _chk(resized); _chk(add); _chk(matte)
+    N, Cc, H, W = resized.shape
+    assert Cc == 3 and add.shape == resized.shape and tuple(matte.shape) == (N, 1, H, W), (resized.shape, add.shape, matte.shape)
+    if face is not None:
+        _chk(face, torch.uint8)
+        assert tuple(face.shape) == (N, 1, H, W), face.shape
+    if out is None:
+        out = torch.empty_like(resized)
+    if u8 is None:
+        u8 = torch.empty((N, H, W, 3), dtype=torch.uint8, device=resized.device)
+    _chk(out); _chk(u8, torch.uint8)
+    assert out.shape == resized.shape and tuple(u8.shape) == (N, H, W, 3), (out.shape, u8.shape)
+    L.call("emo_s2_finish_masked", _p(resized), _p(add), _p(matte), _p(face), N, H, W, _p(out), _p(u8), _stream())
+    return out, u8
+
+
 def s2_finish(resized: torch.Tensor, add: torch.Tensor, out: Optional[torch.Tensor] = None,
               u8: Optional[torch.Tensor] = None):
     """(ffhq, u8): ffhq = (resized + add).clamp_(0, 1) (N,3,H,W) fp32 and u8 = image_to_u8(ffhq) (N,H,W,3), in one pass"""

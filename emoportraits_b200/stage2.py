@@ -20,7 +20,7 @@ from typing import Optional
 
 import torch
 
-from . import nets, ops
+from . import masks, nets, ops
 from .checkpoint import _fill, _sn
 from .config import parse_args
 
@@ -217,15 +217,18 @@ class Stage2Model:
         return out[:, :, 0]
 
     @torch.no_grad()
+    def resize(self, img: torch.Tensor):
+        """the bilinear resize (align_corners=False) of img (N,3,h,w) to the output size, both as the encoder's channels-last
+        input x4 (N,1,S,S,4), 4th channel 0, and as the NCHW tensor (N,3,S,S) the residual is added to: (x4, resized)"""
+        S = self.cfg.output_size
+        x4 = ops.resize_bilinear(img.contiguous().float(), (S, S))
+        return x4, x4[:, 0, :, :, :3].permute(0, 3, 1, 2).contiguous()
+
+    @torch.no_grad()
     def forward(self, img: torch.Tensor, mask: Optional[torch.Tensor] = None, face_mask: Optional[torch.Tensor] = None):
         """notebooks/infer_s2.py:351-376.  img (N,3,h,w) in [0,1] on device.  Masks default to ones (MODNet / BiSeNet are
         out of scope).  Returns (resized, add, ffhq) NCHW fp32."""
-        S = self.cfg.output_size
-        img = img.contiguous().float()
-        N = img.shape[0]
-        # bilinear resize (align_corners=False) both as the NCHW tensor the residual is added to and as the encoder input
-        x4 = ops.resize_bilinear(img, (S, S))                                   # (N,1,S,S,4) channels-last, 4th channel 0
-        resized = x4[:, 0, :, :, :3].permute(0, 3, 1, 2).contiguous()
+        x4, resized = self.resize(img)
         if mask is not None:
             x4 = (x4 * mask.to(self.device).float().permute(0, 2, 3, 1)[:, None]).contiguous()
         add = self.decoder(self.local_encoder(x4))
@@ -237,15 +240,37 @@ class Stage2Model:
         return resized, add, ffhq
 
     @torch.no_grad()
-    def refine(self, img: torch.Tensor, out: Optional[torch.Tensor] = None, u8: Optional[torch.Tensor] = None):
-        """forward(img)'s ffhq without masks, as kernels only, so that a CUDA graph can capture it after a stage-1 frame:
-        ops.s2_prepare (the resize and the stem's operand in one pass) -> the encoder and decoder convolutions forward
-        runs -> ops.s2_finish (clamp(resized + add, 0, 1) and its uint8 frame in one pass).  img (N,3,h,w) fp32 contiguous
-        on the device.  out (N,3,S,S) fp32 / u8 (N,S,S,3) uint8: written in place if given.  Returns (resized, ffhq, u8),
-        bit-identical to forward(img)'s resized and ffhq and to ops.image_to_u8(ffhq)."""
-        resized, stem_in = ops.s2_prepare(img, self.cfg.output_size, fast=self.stem_h1 is not None)
+    def refine(self, img: torch.Tensor, out: Optional[torch.Tensor] = None, u8: Optional[torch.Tensor] = None, modnet=None,
+               face_idt=None, cloth: bool = False, matte: Optional[torch.Tensor] = None, bg: Optional[torch.Tensor] = None,
+               threshold: float = 0.3):
+        """forward(img)'s ffhq as kernels and the caller's mask networks only, so that a CUDA graph can capture it after a
+        stage-1 frame: ops.s2_prepare (the resize and the stem's operand in one pass) -> the encoder and decoder convolutions
+        forward runs -> ops.s2_finish (clamp(resized + add, 0, 1) and its uint8 frame in one pass).  img (N,3,h,w) fp32
+        contiguous on the device.  out (N,3,S,S) fp32 / u8 (N,S,S,3) uint8: written in place if given.
+        matte (N,1,h,w) + bg (3,h,w): img is first composited over bg as video.connect_img_and_bg does (ops.s2_prepare_composite,
+        the composited image never in memory).
+        modnet (the matting network), face_idt (a masks.FaceParsing or None) and cloth: stage 2's masks, as
+        InferenceWrapper.forward computes them with these networks plugged in: the matte of `resized` (masks.modnet_get_mask)
+        masks the stem's input (ops.s2_masked_stem), and the matte times the face mask (face_idt.label_masks, kept as uint8;
+        the matte alone with cloth or without face_idt) masks the residual (ops.s2_finish_masked).
+        Returns (resized, ffhq, u8), bit-identical to forward(x, mask, face_mask)'s resized and ffhq with the same masks, x the
+        (composited) image, and to ops.image_to_u8(ffhq)."""
+        S, fast = self.cfg.output_size, self.stem_h1 is not None
+        if bg is not None:
+            resized, stem_in = ops.s2_prepare_composite(img, matte.contiguous().float(), bg, S, None if modnet is not None else fast,
+                                                        threshold)
+        else:
+            resized, stem_in = ops.s2_prepare(img, S, fast=fast)
+        if modnet is None:
+            add = self.decoder(self._encode(stem_in))
+            ffhq, u8 = ops.s2_finish(resized, add, out=out, u8=u8)
+            return resized, ffhq, u8
+        rmatte = masks.modnet_get_mask(modnet, resized).contiguous()
+        face = None if cloth or face_idt is None else face_idt.label_masks(resized)[0]
+        # without a composite the prepare pass wrote the unmasked operand: the masked one overwrites it
+        stem_in = ops.s2_masked_stem(resized, rmatte, fast, out=stem_in)
         add = self.decoder(self._encode(stem_in))
-        ffhq, u8 = ops.s2_finish(resized, add, out=out, u8=u8)
+        ffhq, u8 = ops.s2_finish_masked(resized, add, rmatte, face, out=out, u8=u8)
         return resized, ffhq, u8
 
 
@@ -276,15 +301,40 @@ class InferenceWrapper(torch.nn.Module):
             state_dict = torch.load(self.model_checkpoint_s2, map_location='cpu')
         self.precision = precision
         self.model_two = Stage2Model(self.cfg, state_dict, self.device, precision=precision)
+        # the external mask networks (separate checkouts in the reference: MODNet behind self.modnet, infer_s2.py:134-143, and
+        # BiSeNet behind self.face_idt, :71): plug them in as `wrapper.modnet = <module>` /
+        # `wrapper.face_idt = masks.FaceParsing(None, net=...)`
+        self.modnet = None
+        self.face_idt = None
+
+    def check_masks(self) -> None:
+        """ValueError unless the plugged-in mask networks are a set forward can use: face_idt needs modnet (the reference's
+        residual mask is the matte times the face mask)"""
+        if self.face_idt is not None and self.modnet is None:
+            raise ValueError("stage 2's face mask multiplies the MODNet matte: plug in wrapper.modnet together with wrapper.face_idt")
 
     @torch.no_grad()
     def forward(self, img, cloth=False, mask=None, face_mask=None):
+        """infer_s2.py:351-376.  img (N,3,h,w) in [0,1].  Returns (pil, pil_resized, pil_ffhq, mask).
+        mask (N,1,S,S) / face_mask (N,1,S,S), given by the caller: the stem's input is resized * mask and the residual is
+        multiplied by mask * face_mask.  Given neither, with the networks plugged in (modnet, face_idt): the reference's
+        masks, computed on the resized image (mask = modnet_get_mask(modnet, resized), face_mask = face_idt.forward(resized)[0],
+        no face mask with cloth=True), and the fourth output is the matte of img clamped to [0, 1].  Without networks and
+        masks stage 2 runs unmasked and the fourth output is ones."""
         from PIL import Image
 
         img = img.to(self.device).float()
+        pred_mask = None
+        if mask is None and face_mask is None and self.modnet is not None:
+            self.check_masks()
+            pred_mask = masks.modnet_get_mask(self.modnet, img)                             # :356
+            _, resized = self.model_two.resize(img)                                         # :360
+            mask = masks.modnet_get_mask(self.modnet, resized)                              # :361
+            if self.face_idt is not None:
+                face_mask = self.face_idt.forward(resized)[0]                               # :362
         if self.cloth:
             face_mask = None  # infer_s2.py:365-368: with cloth=True the refinement is not restricted to the face region
         resized, add, ffhq = self.model_two.forward(img, mask, face_mask)
         to_pil = lambda t: [Image.fromarray(h) for h in ops.image_to_u8(t.detach().contiguous().float()).cpu().numpy()]
-        m = mask if mask is not None else torch.ones_like(img[:, :1])
+        m = pred_mask if pred_mask is not None else mask if mask is not None else torch.ones_like(img[:, :1])
         return to_pil(img), to_pil(resized), to_pil(ffhq), m.detach().cpu().clamp(0, 1)

@@ -49,7 +49,7 @@ def connect_img_and_bg(img: torch.Tensor, bg: torch.Tensor, mask: torch.Tensor, 
 
 def drive_image_with_video(inferer, source, frames: Sequence, inferer_s2=None, bg: Optional[torch.Tensor] = None,
                            mask_fn: Optional[Callable[[torch.Tensor], torch.Tensor]] = None, chunk: int = 16,
-                           crop_box: Optional[tuple] = None):
+                           crop_box: Optional[tuple] = None, in_flight: bool = False):
     """cell 51.  `inferer`: stage-1 InferenceWrapper, `inferer_s2`: stage-2 wrapper or None, `source`: PIL image, `frames`:
     driving frames (PIL).  Returns (list of output PIL images, list of cropped PIL images or None, frames).
     bg (3,H,W) tensor + mask_fn: composite every animated frame over the background (cell 41) before stage 2.
@@ -57,9 +57,16 @@ def drive_image_with_video(inferer, source, frames: Sequence, inferer_s2=None, b
     caller's face detector).
     Each wrapper runs with the `precision=` it was built with: a stage-2 wrapper built with precision="fast" refines every
     chunk in fast mode, exactly as calling that wrapper on the same chunk would.  A stage-1 wrapper built with
-    source_precision="fast" runs the one source pass in fast mode, and every frame reads that cached source volume."""
+    source_precision="fast" runs the one source pass in fast mode, and every frame reads that cached source volume.
+    in_flight=True (needs inferer_s2): every frame runs stage 1, the composite (with bg and mask_fn) and stage 2 with the masks
+    of the networks plugged into inferer_s2 in one captured graph, with frames in flight (InferenceWrapper.forward_refined),
+    `chunk` frames per call; the fixed crop is applied afterwards.  The default (False) runs stage 2 eagerly on each chunk
+    as a batch.  Both paths keep the float images between the steps: the notebook rounds every step to uint8 (PIL) before
+    the next, this function does not, on either path."""
     from PIL import Image
 
+    if in_flight and inferer_s2 is None:
+        raise ValueError("in_flight=True refines the frames in flight: it needs inferer_s2")
     kw = dict(crop=False, smooth_pose=False, target_theta=True, mix=True, mix_old=False, modnet_mask=False)
     outs: List[Image.Image] = []
     frames = list(frames)
@@ -67,16 +74,23 @@ def drive_image_with_video(inferer, source, frames: Sequence, inferer_s2=None, b
         return [], None if crop_box is None else [], frames
     inferer.forward(source, None, **kw)                       # source pass once (the notebook folds it into the first call)
     dev = inferer.device
-    for i in range(0, len(frames), chunk):
-        part = frames[i:i + chunk]
-        _, img = inferer.forward(None, part, **kw)            # (n,3,H,W) on the device, frames pipelined in flight
-        if bg is not None and mask_fn is not None:
-            img = connect_img_and_bg(img, bg.to(dev), mask_fn(img))
-        if inferer_s2 is not None:
-            _, _, s2, _ = inferer_s2.forward(img)             # batch of n through the refinement encoder/decoder
-            outs.extend(s2)
-        else:
-            outs.extend(Image.fromarray(h) for h in ops.image_to_u8(img.contiguous()).cpu().numpy())
+    composite = bg is not None and mask_fn is not None
+    if in_flight:
+        for i in range(0, len(frames), chunk):
+            pil, _ = inferer.forward_refined(frames[i:i + chunk], inferer_s2, mix=True, target_theta=True, mix_old=False,
+                                             bg=bg if composite else None, mask_fn=mask_fn if composite else None)
+            outs.extend(pil)
+    else:
+        for i in range(0, len(frames), chunk):
+            part = frames[i:i + chunk]
+            _, img = inferer.forward(None, part, **kw)            # (n,3,H,W) on the device, frames pipelined in flight
+            if composite:
+                img = connect_img_and_bg(img, bg.to(dev), mask_fn(img))
+            if inferer_s2 is not None:
+                _, _, s2, _ = inferer_s2.forward(img)             # batch of n through the refinement encoder/decoder
+                outs.extend(s2)
+            else:
+                outs.extend(Image.fromarray(h) for h in ops.image_to_u8(img.contiguous()).cpu().numpy())
     crops = None
     if crop_box is not None:
         size = outs[0].size

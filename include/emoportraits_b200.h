@@ -35,7 +35,7 @@ extern "C" {
 enum { EMO_ACT_NONE = 0, EMO_ACT_RELU = 1, EMO_ACT_SIGMOID = 2, EMO_ACT_TANH = 3 };
 
 const char* emo_last_error(void);
-int emo_version(void); /* 108: + emo_s2_prepare, emo_s2_finish; 107: + emo_stem_pack; 106: one-plane fp16 operands (emo_conv_desc, emo_apply_desc, emo_grid_sample3d_desc.plane_fp16,
+int emo_version(void); /* 109: + emo_s2_prepare_composite, emo_s2_masked_stem, emo_s2_finish_masked; 108: + emo_s2_prepare, emo_s2_finish; 107: + emo_stem_pack; 106: one-plane fp16 operands (emo_conv_desc, emo_apply_desc, emo_grid_sample3d_desc.plane_fp16,
                           emo_split_f16 with lo == NULL) and the EMO_CONV_KERNEL_H1_* kernels; 105: + emo_conv_plan; 104: + emo_composite; 103: emo_conv_desc.post; 102: + emo_u8_to_image, emo_image_to_u8, emo_resize_bicubic; 101: emo_pose_desc and emo_conv_desc gained trailing fields */
 /* sm count, and cc major*10+minor of the current device */
 int emo_device_info(int* sm_count, int* cc);
@@ -411,6 +411,22 @@ int emo_resize_bicubic(const float* in, int N, int C, int Hin, int Win, int Hout
 int emo_s2_prepare(const float* img, int N, int Hin, int Win, int S, float* resized, float* x4, void* plane, float plane_scale,
                    void* stream);
 int emo_s2_finish(const float* resized, const float* add, int N, int H, int W, float* out, unsigned char* u8, void* stream);
+/* The same handoff with the stage-2 masks of notebooks/infer_s2.py:356-376 and the video loop's composite (E_emo_infer_video.ipynb
+ * cell 41), each bit for bit the eager composition it replaces:
+ *   emo_s2_prepare_composite  emo_s2_prepare of emo_composite(img, matte, bg, threshold) (img fp32 [N][3][Hin][Win], matte fp32
+ *                             [N][1][Hin][Win], bg fp32 [3][Hin][Win]); the composited image never exists in memory.  At most one
+ *                             stem operand: none when the stem reads a masked operand (emo_s2_masked_stem).
+ *   emo_s2_masked_stem        the stem's operand of resized * matte (resized fp32 [N][3][S][S], matte fp32 [N][1][S][S]):
+ *                             exactly one of x4 (R m, G m, B m, 0 m) fp32 [N][S][S][4] or emo_stem_pack's plane of that x4,
+ *                             16-byte aligned.
+ *   emo_s2_finish_masked      emo_s2_finish with the residual masked: out = clamp(resized + add * (matte * face), 0, 1), one fp32
+ *                             rounding per operation, a NaN stays NaN; matte fp32 [N][1][H][W], face uint8 0 / 1 [N][1][H][W] (the
+ *                             first mask of emo_parsing_masks) or NULL for matte alone; u8 as emo_s2_finish. */
+int emo_s2_prepare_composite(const float* img, const float* matte, const float* bg, float threshold, int N, int Hin, int Win, int S,
+                             float* resized, float* x4, void* plane, float plane_scale, void* stream);
+int emo_s2_masked_stem(const float* resized, const float* matte, int N, int S, float* x4, void* plane, float plane_scale, void* stream);
+int emo_s2_finish_masked(const float* resized, const float* add, const float* matte, const unsigned char* face, int N, int H, int W,
+                         float* out, unsigned char* u8, void* stream);
 /* Foreground / background compositing of the video loop (notebooks/E_emo_infer_video.ipynb cell 41, connect_img_and_bg):
  *   m' = (mask > threshold ? mask : 0)^8;  out = m' * img + (1 - m') * bg
  * img, out fp32 [N][C][H][W]; mask fp32 [N][1][H][W]; bg fp32 [C][H][W] (one background for the whole clip). */
