@@ -376,7 +376,7 @@ extern "C" int emo_composite(const float* img, const float* mask, const float* b
 }
 
 extern "C" const char* emo_last_error(void) { return emo::g_err; }
-extern "C" int emo_version(void) { return 109; }  // 101: emo_pose_desc (+theta_in, mix_old, smoothing) and emo_conv_desc (+upconv) grew trailing fields
+extern "C" int emo_version(void) { return 110; }  // 101: emo_pose_desc (+theta_in, mix_old, smoothing) and emo_conv_desc (+upconv) grew trailing fields
 
 extern "C" int emo_device_info(int* sm_count, int* cc) {
   int dev = 0;

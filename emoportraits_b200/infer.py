@@ -813,24 +813,7 @@ class InferenceWrapper(torch.nn.Module):
         (RuntimeError), a stage-2 wrapper on another device, mask networks or inputs that do not fit (ValueError)."""
         if self._state is None:
             raise RuntimeError("forward_refined() called before a source image was given")
-        s2 = getattr(inferer_s2, "model_two", None)
-        if s2 is None:
-            raise ValueError("inferer_s2 must be a stage2.InferenceWrapper")
-        if (bg is None) != (mask_fn is None):
-            raise ValueError("bg and mask_fn composite the frames together: give both, or neither")
-        extra = {}
-        modnet, face_idt = getattr(inferer_s2, "modnet", None), getattr(inferer_s2, "face_idt", None)
-        if modnet is not None or face_idt is not None:
-            extra["refine_masks"] = dict(modnet=modnet, face_idt=face_idt, cloth=bool(getattr(inferer_s2, "cloth", False)))
-        if mask_fn is not None:
-            extra["composite"] = mask_fn
-            s = self.cfg.image_size
-            bg = torch.as_tensor(bg)
-            if tuple(bg.shape) != (3, s, s) or not bg.is_floating_point():
-                raise ValueError(f"bg must be a floating-point background of shape {(3, s, s)}, got {tuple(bg.shape)} {bg.dtype}")
-            bg = bg.to(self.device, torch.float32).contiguous()
-        self.model.check_refine(s2, encode=False)
-        Model.check_refine_masks(s2, extra.get("refine_masks"), mask_fn)
+        s2, extra, bg = self._refining_options(inferer_s2, bg, mask_fn)
         with_bg = (lambda kw: dict(kw, bg=bg)) if bg is not None else (lambda kw: kw)
         E = self.cfg.expr_channels
         if driver_images is None:
@@ -862,6 +845,29 @@ class InferenceWrapper(torch.nn.Module):
         n, frame = self._frames(driver_images)
         pipe = self._driver_pipeline(mix, target_theta, mix_old, refine=s2, **extra, theta_embed=srt is not None, pose_embed=pe is not None)
         return self._render(pipe, n, lambda i: with_bg(dict(drv=frame(i), theta_embed=srt, pose_embed=pe)))
+
+    def _refining_options(self, inferer_s2, bg, mask_fn):
+        """forward_refined's checks of a stage-2 wrapper, its mask networks and a composite: (the stage-2 model, the
+        _driver_pipeline options refine_masks= / composite=, bg as a float32 device tensor or None); ValueError if they do not fit"""
+        s2 = getattr(inferer_s2, "model_two", None)
+        if s2 is None:
+            raise ValueError("inferer_s2 must be a stage2.InferenceWrapper")
+        if (bg is None) != (mask_fn is None):
+            raise ValueError("bg and mask_fn composite the frames together: give both, or neither")
+        extra = {}
+        modnet, face_idt = getattr(inferer_s2, "modnet", None), getattr(inferer_s2, "face_idt", None)
+        if modnet is not None or face_idt is not None:
+            extra["refine_masks"] = dict(modnet=modnet, face_idt=face_idt, cloth=bool(getattr(inferer_s2, "cloth", False)))
+        if mask_fn is not None:
+            extra["composite"] = mask_fn
+            s = self.cfg.image_size
+            bg = torch.as_tensor(bg)
+            if tuple(bg.shape) != (3, s, s) or not bg.is_floating_point():
+                raise ValueError(f"bg must be a floating-point background of shape {(3, s, s)}, got {tuple(bg.shape)} {bg.dtype}")
+            bg = bg.to(self.device, torch.float32).contiguous()
+        self.model.check_refine(s2, encode=False)
+        Model.check_refine_masks(s2, extra.get("refine_masks"), mask_fn)
+        return s2, extra, bg
 
     # -- notebooks/infer.py:229-243
     def convert_to_tensor(self, image):

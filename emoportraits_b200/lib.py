@@ -151,6 +151,9 @@ SYMBOLS = {
     "emo_parsing_prepare": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "emo_parsing_masks": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "emo_resize_area": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_float, c_void_p, c_void_p]),
+    "emo_resample_u8": (c_int, [c_void_p, c_int, c_int, c_ll, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int, c_int, c_ll, c_int,
+                                c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p]),
+    "emo_mask_dilate": (c_int, [c_void_p, c_int, c_int, c_int, c_float, c_int, c_void_p, c_void_p, c_void_p]),
 }
 
 # EMO_DRY_RUN=1: host-logic test mode for the GPU-less CI box — every C-ABI call is validated for presence in the

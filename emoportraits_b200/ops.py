@@ -8,6 +8,8 @@ Layout vocabulary
 from __future__ import annotations
 
 import ctypes as C
+import math
+import numbers
 from dataclasses import dataclass
 from typing import Optional
 
@@ -839,4 +841,140 @@ def resize_area(img_nchw: torch.Tensor, out_hw, scale: float = 1.0, shift: float
     N, Cc, Hi, Wi = img_nchw.shape
     out = torch.empty((N, Cc, out_hw[0], out_hw[1]), dtype=torch.float32, device=img_nchw.device)
     L.call("emo_resize_area", _p(img_nchw), N, Cc, Hi, Wi, out_hw[0], out_hw[1], float(scale), float(shift), _p(out), _stream())
+    return out
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# image plumbing of the demo video loop (csrc/video.cu)
+# ------------------------------------------------------------------------------------------------------------------
+def _sinc(x: float) -> float:
+    if x == 0.0:
+        return 1.0
+    x = x * math.pi
+    return math.sin(x) / x
+
+
+def _lanczos(x: float) -> float:
+    return _sinc(x) * _sinc(x / 3) if -3.0 <= x < 3.0 else 0.0
+
+
+def _bicubic(x: float) -> float:
+    a = -0.5
+    if x < 0.0:
+        x = -x
+    if x < 1.0:
+        return ((a + 2.0) * x - (a + 3.0)) * x * x + 1
+    if x < 2.0:
+        return (((x - 5) * x + 8) * x - 4) * a
+    return 0.0
+
+
+# Pillow's LANCZOS and BICUBIC filters (libImaging/Resample.c) with their supports: the only two the video loop uses
+RESAMPLE_FILTERS = {"lanczos": (_lanczos, 3.0), "bicubic": (_bicubic, 2.0)}
+RESAMPLE_BITS = 22   # Pillow's PRECISION_BITS: fixed-point coefficients of uint8 resizes
+
+
+def resample_coeffs(in_size: int, out_size: int, filter: str):
+    """Pillow's fixed-point taps of a resize of one axis from in_size to out_size (precompute_coeffs over the box (0, in_size),
+    then normalize_coeffs_8bpc): a list of (first tap, [coefficients]) per output index.  Python floats and math.sin are the
+    IEEE double operations and the libm of Pillow's C code, so these are Pillow's integers."""
+    fn, support = RESAMPLE_FILTERS[filter]
+    scale = in_size / out_size
+    fs = max(scale, 1.0)
+    support = support * fs
+    ss = 1.0 / fs
+    one = 1 << RESAMPLE_BITS
+    taps = []
+    for xx in range(out_size):
+        center = (xx + 0.5) * scale
+        xmin = max(int(center - support + 0.5), 0)
+        n = min(int(center + support + 0.5), in_size) - xmin
+        k = [fn((x + xmin - center + 0.5) * ss) for x in range(n)]
+        ww = 0.0
+        for w in k:
+            ww += w
+        if ww != 0.0:
+            k = [w / ww for w in k]
+        taps.append((xmin, [int(-0.5 + w * one) if w < 0 else int(0.5 + w * one) for w in k]))
+    return taps
+
+
+@dataclass
+class ResampleTaps:
+    """resample_coeffs() of one axis on the device as emo_resample_u8 reads it: int32 (out, 2 + kmax) rows of (first tap, tap
+    count, coefficients); lo / hi: the first and one past the last input index any output reads (Pillow's ybox)."""
+    table: torch.Tensor
+    kmax: int
+    lo: int
+    hi: int
+
+
+_RESAMPLE_TAPS = {}
+
+
+def resample_taps(in_size: int, out_size: int, filter: str, device) -> ResampleTaps:
+    """The cached device taps of (in_size -> out_size, filter).  The first call builds and uploads them, so a caller that
+    captures resample_u8 calls this for its shapes first: a captured launch must not copy from the host."""
+    if filter not in RESAMPLE_FILTERS:
+        raise ValueError(f"filter={filter!r}: one of {sorted(RESAMPLE_FILTERS)}")
+    key = (int(in_size), int(out_size), filter, _dev_key(device))
+    t = _RESAMPLE_TAPS.get(key)
+    if t is None:
+        coeffs = resample_coeffs(int(in_size), int(out_size), filter)
+        kmax = max(len(k) for _, k in coeffs)
+        rows = [[first, len(k)] + k + [0] * (kmax - len(k)) for first, k in coeffs]
+        table = torch.tensor(rows, dtype=torch.int32)
+        t = ResampleTaps(table if L.DRY_RUN else table.to(device), kmax, coeffs[0][0], coeffs[-1][0] + len(coeffs[-1][1]))
+        _RESAMPLE_TAPS[key] = t
+    return t
+
+
+def _u8_image(t: torch.Tensor, what: str):
+    """(H, W, 3) uint8 on the device with rows of any pitch and packed pixels -> its row pitch in bytes"""
+    assert (t.is_cuda or L.DRY_RUN) and t.dtype == torch.uint8 and t.dim() == 3 and t.shape[2] == 3, (what, t.shape, t.dtype)
+    assert t.stride(2) == 1 and t.stride(1) == 3 and t.stride(0) >= 3 * t.shape[1], (what, t.stride())
+    return t.stride(0)
+
+
+def resample_u8(src: torch.Tensor, size, filter: str, crop=None, dst: Optional[torch.Tensor] = None, src_bgr: bool = False,
+                dst_bgr: bool = False) -> torch.Tensor:
+    """Pillow's Image.crop(crop).resize(size, filter) of a (H, W, 3) uint8 image on the device, bit for bit: filter "lanczos"
+    (Image.LANCZOS) or "bicubic" (Image.BICUBIC), size = (width, height) as Pillow takes it, crop = integer (left, upper,
+    right, lower) or None for the whole image; pixels outside the source read as 0.  src and dst may be views with any row
+    pitch (a panel of a wider row); src_bgr / dst_bgr give each side's channel order.  Returns dst, (height, width, 3)."""
+    sp = _u8_image(src, "src")
+    H, W = src.shape[:2]
+    x0, y0, x1, y1 = (0, 0, W, H) if crop is None else tuple(crop)
+    if not all(isinstance(v, numbers.Integral) for v in (x0, y0, x1, y1)) or x1 <= x0 or y1 <= y0:
+        raise ValueError(f"crop must be a non-empty box of integers (left, upper, right, lower), got {crop}")
+    ow, oh = int(size[0]), int(size[1])
+    if ow <= 0 or oh <= 0:
+        raise ValueError(f"size must be positive (width, height), got {size}")
+    cw, ch = x1 - x0, y1 - y0
+    if dst is None:
+        dst = torch.empty((oh, ow, 3), dtype=torch.uint8, device=src.device)
+    dp = _u8_image(dst, "dst")
+    assert tuple(dst.shape[:2]) == (oh, ow), (dst.shape, size)
+    ht = resample_taps(cw, ow, filter, src.device) if ow != cw else None
+    vt = resample_taps(ch, oh, filter, src.device) if oh != ch else None
+    tmp, t0, rows = None, 0, 0
+    if ht is not None and vt is not None:
+        t0, rows = vt.lo, vt.hi - vt.lo
+        tmp = torch.empty((rows, ow, 3), dtype=torch.uint8, device=src.device)
+    x0, y0 = int(x0), int(y0)
+    L.call("emo_resample_u8", _p(src), H, W, sp, int(src_bgr), x0, y0, cw, ch, _p(dst), oh, ow, dp, int(dst_bgr),
+           _p(ht.table) if ht else None, ht.kmax if ht else 0, _p(vt.table) if vt else None, vt.kmax if vt else 0, _p(tmp), t0, rows,
+           _stream())
+    return dst
+
+
+def mask_dilate(m: torch.Tensor, thr: float, radius: int) -> torch.Tensor:
+    """max over a (2 radius + 1)^2 window, clipped to the image, of (m >= thr): m (N,1,H,W) fp32 -> (N,1,H,W) fp32 0 / 1.  With
+    radius 20 this is the notebook's cv2.dilate((m >= thr).float(), ones(21, 21), iterations=2) (cell 40)."""
+    _chk(m)
+    N, Cc, H, W = m.shape
+    assert Cc == 1, m.shape
+    out = torch.empty_like(m)
+    tmp = torch.empty((N, H, W), dtype=torch.uint8, device=m.device)
+    L.call("emo_mask_dilate", _p(m), N, H, W, C.c_float(thr), int(radius), _p(tmp), _p(out), _stream())
     return out

@@ -35,7 +35,7 @@ extern "C" {
 enum { EMO_ACT_NONE = 0, EMO_ACT_RELU = 1, EMO_ACT_SIGMOID = 2, EMO_ACT_TANH = 3 };
 
 const char* emo_last_error(void);
-int emo_version(void); /* 109: + emo_s2_prepare_composite, emo_s2_masked_stem, emo_s2_finish_masked; 108: + emo_s2_prepare, emo_s2_finish; 107: + emo_stem_pack; 106: one-plane fp16 operands (emo_conv_desc, emo_apply_desc, emo_grid_sample3d_desc.plane_fp16,
+int emo_version(void); /* 110: + emo_resample_u8, emo_mask_dilate; 109: + emo_s2_prepare_composite, emo_s2_masked_stem, emo_s2_finish_masked; 108: + emo_s2_prepare, emo_s2_finish; 107: + emo_stem_pack; 106: one-plane fp16 operands (emo_conv_desc, emo_apply_desc, emo_grid_sample3d_desc.plane_fp16,
                           emo_split_f16 with lo == NULL) and the EMO_CONV_KERNEL_H1_* kernels; 105: + emo_conv_plan; 104: + emo_composite; 103: emo_conv_desc.post; 102: + emo_u8_to_image, emo_image_to_u8, emo_resize_bicubic; 101: emo_pose_desc and emo_conv_desc gained trailing fields */
 /* sm count, and cc major*10+minor of the current device */
 int emo_device_info(int* sm_count, int* cc);
@@ -449,6 +449,26 @@ int emo_parsing_masks(const float* logits, int N, int K, int Hin, int Win, int H
                       unsigned char* out, unsigned char* labels, void* stream);
 int emo_resize_area(const float* in, int N, int C, int Hin, int Win, int Hout, int Wout, float scale, float shift, float* out,
                     void* stream);
+/* ------------------------------------------------------------------------------------------------
+ * Image plumbing of the demo video loop (E_emo_infer_video.ipynb cells 40, 46-49)
+ *   emo_resample_u8  Pillow's Image.crop((x0, y0, x0 + crop_w, y0 + crop_h)).resize((out_w, out_h), f), bit for bit, for an
+ *                    interleaved 3-channel uint8 image (LANCZOS or BICUBIC: the filter lives in the taps).  src [src_h] rows
+ *                    of src_pitch bytes, dst [out_h] rows of dst_pitch bytes (a column offset is a pointer offset); *_bgr
+ *                    give each side's channel order, so a BGR frame is read and a BGR video row written directly.  Pixels
+ *                    outside the source read as 0 (Image.crop's padding).  h_taps / v_taps: per output column / row, one
+ *                    row of (2 + kmax) ints: first tap in crop coordinates, tap count, then the coefficients with 22
+ *                    fractional bits (Pillow's precompute_coeffs + normalize_coeffs_8bpc); NULL exactly for an axis whose
+ *                    size does not change (Pillow skips that pass; with both NULL the call is a copy).  With both passes
+ *                    the horizontal one writes crop rows tmp_y0 .. tmp_y0 + tmp_rows (the rows the vertical taps read) to
+ *                    tmp [tmp_rows][out_w][3].  replaces the PIL resizes of cells 46-49.
+ *   emo_mask_dilate  out = max over the (2 radius + 1)^2 window, clipped to the image, of (m >= thr); m, out fp32
+ *                    [N][H][W], out 0 / 1, tmp uint8 [N][H][W].  replaces cell 40's cv2.dilate((m >= 0.8), ones(21, 21),
+ *                    iterations=2) (radius 20).
+ * ------------------------------------------------------------------------------------------------ */
+int emo_resample_u8(const unsigned char* src, int src_h, int src_w, long long src_pitch, int src_bgr, int x0, int y0, int crop_w,
+                    int crop_h, unsigned char* dst, int out_h, int out_w, long long dst_pitch, int dst_bgr, const int* h_taps,
+                    int h_kmax, const int* v_taps, int v_kmax, unsigned char* tmp, int tmp_y0, int tmp_rows, void* stream);
+int emo_mask_dilate(const float* m, int N, int H, int W, float thr, int radius, unsigned char* tmp, float* out, void* stream);
 /* L2 flush helpers for benchmarks: emo_l2_flush writes `bytes` of `buf` (L2 is left full of DIRTY foreign lines: the next
  * kernel also pays for their write-back); emo_l2_flush_clean writes and then reads the buffer back (L2 is left full of
  * CLEAN foreign lines). */
