@@ -376,7 +376,7 @@ extern "C" int emo_composite(const float* img, const float* mask, const float* b
 }
 
 extern "C" const char* emo_last_error(void) { return emo::g_err; }
-extern "C" int emo_version(void) { return 110; }  // 101: emo_pose_desc (+theta_in, mix_old, smoothing) and emo_conv_desc (+upconv) grew trailing fields
+extern "C" int emo_version(void) { return 111; }  // 101: emo_pose_desc (+theta_in, mix_old, smoothing) and emo_conv_desc (+upconv) grew trailing fields
 
 extern "C" int emo_device_info(int* sm_count, int* cc) {
   int dev = 0;
@@ -485,6 +485,14 @@ extern "C" int emo_pose_theta(const emo_pose_desc* d, void* stream_) {
   EMO_REQUIRE(!d->mix || d->source_theta, "emo_pose_theta: mix needs source_theta");
   EMO_REQUIRE(!d->smooth_state || (d->smooth_momentum >= 0.f && d->smooth_momentum <= 1.f),
               "emo_pose_theta: smooth_momentum must be in [0,1]");
+  EMO_REQUIRE(!d->smooth_state || (d->smooth_one_minus >= 0.f && d->smooth_one_minus <= 1.f),
+              "emo_pose_theta: smooth_one_minus must be in [0,1]");
+  // a value that does not belong to the momentum would smooth with the wrong weights; fp32(1 - m) and 1 - fp32(m) differ
+  // by under 2^-23.  Zero stands for "derive it from smooth_momentum" (pose_math.cuh)
+  EMO_REQUIRE(!d->smooth_state || d->smooth_one_minus == 0.f ||
+                  fabs((double)d->smooth_one_minus - (1.0 - (double)d->smooth_momentum)) <= 0x1p-23,
+              "emo_pose_theta: smooth_one_minus must be 1 - smooth_momentum (%.9g, %.9g)", d->smooth_one_minus,
+              d->smooth_momentum);
   launch_kernel(pose_theta_kernel, cdiv(d->N, 32), 32, 0, stream, *d);
   return check_launch("emo_pose_theta");
 }

@@ -175,8 +175,11 @@ EMO_HD inline void pose_sample(const emo_pose_desc& d, int n) {
   if (d.mix) mix_theta(d.source_theta, d.mix_old, th);
   if (d.smooth_state) {
     // self.theta = theta_i * m + self.theta * (1 - m) on rows [:3]; the first frame after a reset seeds the state
-    // (notebooks/infer.py:572-577).  Python evaluates 1 - m in double; the product takes it rounded to fp32.
-    const float m = d.smooth_momentum, om = (float)(1.0 - (double)d.smooth_momentum);
+    // (notebooks/infer.py:572-577).  Python evaluates 1 - m in double from the unrounded momentum and torch rounds the
+    // result to fp32: the caller passes that value, since 1 - fp32(m) rounds differently for momenta like 0.9.  A zero
+    // field is a descriptor that predates it (trailing fields zero-initialised): 1 - fp32(m), which is also 0 at m = 1.
+    const float m = d.smooth_momentum;
+    const float om = d.smooth_one_minus != 0.f ? d.smooth_one_minus : (float)(1.0 - (double)m);
     if (d.smooth_init && n == 0)
       for (int i = 0; i < 12; ++i) d.smooth_state[i] = th[i];
     for (int i = 0; i < 12; ++i) {

@@ -109,7 +109,7 @@ class PoseDesc(C.Structure):
     _fields_ = [("srt", c_void_p), ("source_theta", c_void_p), ("N", c_int), ("mix", c_int), ("invert_warp", c_int),
                 ("theta_out", c_void_p), ("theta_warp", c_void_p), ("align2d", c_void_p),
                 ("theta_in", c_void_p), ("mix_old", c_int), ("smooth_init", c_int), ("smooth_state", c_void_p),
-                ("smooth_momentum", C.c_float)]
+                ("smooth_momentum", C.c_float), ("smooth_one_minus", C.c_float)]
 
 
 # every symbol include/emoportraits_b200.h declares, with its prototype

@@ -662,10 +662,20 @@ def pose_theta(srt: Optional[torch.Tensor], source_theta: Optional[torch.Tensor]
     theta = torch.empty((N, 4, 4), dtype=torch.float32, device=dev)
     warp = torch.empty((N, 3, 4), dtype=torch.float32, device=dev)
     align = torch.empty((N, 2, 3), dtype=torch.float32, device=dev)
-    d = L.PoseDesc(_p(srt), _p(source_theta), N, 1 if mix else 0, 1 if invert_warp else 0, _p(theta), _p(warp), _p(align),
-                   _p(theta_in), 1 if mix_old else 0, 1 if smooth_init else 0, _p(smooth_state), float(smooth_momentum))
+    d = pose_desc(N, _p(srt), _p(source_theta), _p(theta), _p(warp), _p(align), _p(theta_in), _p(smooth_state), mix=mix,
+                  invert_warp=invert_warp, mix_old=mix_old, smooth_init=smooth_init, smooth_momentum=smooth_momentum)
     L.call("emo_pose_theta", C.byref(d), _stream())
     return theta, warp, align
+
+
+def pose_desc(N: int, srt, source_theta, theta_out, theta_warp, align2d, theta_in=None, smooth_state=None, mix=False,
+              invert_warp=False, mix_old=False, smooth_init=False, smooth_momentum: float = 0.5):
+    """emo_pose_desc from raw pointers (int or None).  The state is smoothed as `theta * m + state * (1 - m)` on fp32
+    tensors (notebooks/infer.py:577): torch rounds m to fp32, and 1 - m, evaluated by Python in double, to fp32 as well
+    (as the c_float fields round them here)."""
+    m = float(smooth_momentum)
+    return L.PoseDesc(srt, source_theta, N, 1 if mix else 0, 1 if invert_warp else 0, theta_out, theta_warp, align2d, theta_in,
+                      1 if mix_old else 0, 1 if smooth_init else 0, smooth_state, m, 1.0 - m)
 
 
 def u8_to_image(u8_nhwc: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:

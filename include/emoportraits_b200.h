@@ -35,7 +35,7 @@ extern "C" {
 enum { EMO_ACT_NONE = 0, EMO_ACT_RELU = 1, EMO_ACT_SIGMOID = 2, EMO_ACT_TANH = 3 };
 
 const char* emo_last_error(void);
-int emo_version(void); /* 110: + emo_resample_u8, emo_mask_dilate; 109: + emo_s2_prepare_composite, emo_s2_masked_stem, emo_s2_finish_masked; 108: + emo_s2_prepare, emo_s2_finish; 107: + emo_stem_pack; 106: one-plane fp16 operands (emo_conv_desc, emo_apply_desc, emo_grid_sample3d_desc.plane_fp16,
+int emo_version(void); /* 111: emo_pose_desc.smooth_one_minus; 110: + emo_resample_u8, emo_mask_dilate; 109: + emo_s2_prepare_composite, emo_s2_masked_stem, emo_s2_finish_masked; 108: + emo_s2_prepare, emo_s2_finish; 107: + emo_stem_pack; 106: one-plane fp16 operands (emo_conv_desc, emo_apply_desc, emo_grid_sample3d_desc.plane_fp16,
                           emo_split_f16 with lo == NULL) and the EMO_CONV_KERNEL_H1_* kernels; 105: + emo_conv_plan; 104: + emo_composite; 103: emo_conv_desc.post; 102: + emo_u8_to_image, emo_image_to_u8, emo_resize_bicubic; 101: emo_pose_desc and emo_conv_desc gained trailing fields */
 /* sm count, and cc major*10+minor of the current device */
 int emo_device_info(int* sm_count, int* cc);
@@ -357,9 +357,10 @@ int emo_global_avgpool(const float* x, int N, long long S, int C, float* out, vo
  *   theta = S.R.T (utils/point_transforms.py:187-240), or theta_in when given
  *   mix != 0: get_mixing_theta(source_theta, theta) (infer.py:686-736): polar decompositions in fp64
  *             (scipy.linalg.polar), result rows [:3]; mix_old selects the product of :727 (1) or :729 (0)
- *   smooth_state != NULL: smooth_pose=True (infer.py:571-581): state = theta_n * momentum + state * (1 - momentum)
- *             on rows [:3], sample after sample in order, the state (self.theta) carried across calls in
- *             smooth_state [3][4]; smooth_init != 0 seeds the state with the first sample's theta (self.theta is None)
+ *   smooth_state != NULL: smooth_pose=True (infer.py:571-581): state = theta_n * momentum + state * smooth_one_minus
+ *             (each product rounded to fp32, then the sum) on rows [:3], sample after sample in order, the state
+ *             (self.theta) carried across calls in smooth_state [3][4]; smooth_init != 0 seeds the state with the first
+ *             sample's theta (self.theta is None)
  *   outputs: theta_out [N][4][4]; theta_warp [N][3][4] = (invert ? inverse(theta) : theta)[:3]
  *            (infer.py:443 / :586); align2d [N][2][3] = (inverse(theta4)[[0,1,3]][:, [0,1,3]] . diag(.5,.5,1))[:2]
  *            (expression_embedder.py:176-203).
@@ -378,6 +379,10 @@ typedef struct {
   int smooth_init;       /* with smooth_state: 1 = seed the state with sample 0's theta first */
   float* smooth_state;   /* [3][4] or NULL */
   float smooth_momentum; /* pose_momentum (infer.py:64, default 0.5) */
+  float smooth_one_minus; /* with smooth_state: 1 - pose_momentum as Python computes it (in double, from the unrounded
+                             momentum) rounded to fp32, the factor torch applies to the state; it is not a function of
+                             the fp32 smooth_momentum (0.9 gives 0.1f, 1 - 0.9f rounds 3 ulp above it).  0: not
+                             given, 1 - smooth_momentum in fp32 (a descriptor from before version 111) */
 } emo_pose_desc;
 int emo_pose_theta(const emo_pose_desc* d, void* stream);
 

@@ -2,7 +2,8 @@
 boundary, listed by hand.
 
 A model launch is any C-ABI call of the configurations of model_conv_launches.CONFIGS except emo_conv_igemm (its own table,
-tests/model_conv_launches.json), emo_pose_theta (tests/test_pose_math_host.py) and the benchmark's L2 flushes.  It is stored as
+tests/model_conv_launches.json) and the benchmark's L2 flushes.  The pose algebra's smoothing launches come from the stage-1
+wrapper, not from the models: the smoothing cases of tests/op_cases.py cover them.  It is stored as
 its entry point (`op`), every scalar argument or scalar descriptor field (`args`), the names of its non-NULL pointers (`ptrs`),
 and the variant class and features op_cases.classify gives it.  Launches with equal records are one entry of the table, which
 lists the configurations each came from.  tests/model_op_launches.json is the table of CONFIGS; tests/test_model_op_launches_cpu.py
@@ -33,7 +34,7 @@ import model_conv_launches as MCL  # noqa: E402
 import op_cases as OC  # noqa: E402
 
 CONFIGS = MCL.CONFIGS
-NOT_RECORDED = ("emo_conv_igemm", "emo_pose_theta", "emo_l2_flush", "emo_l2_flush_clean")
+NOT_RECORDED = ("emo_conv_igemm", "emo_l2_flush", "emo_l2_flush_clean")
 SIZE_ARGS = ("N", "H", "W", "Hin", "Win", "Hout", "Wout")   # what `pattern` leaves out
 
 

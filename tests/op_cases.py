@@ -16,6 +16,8 @@ from dataclasses import dataclass
 
 import torch
 
+import pose_reference as PR
+
 SM_COUNT = 132          # H100 SXM
 GS3_CTAS_PER_SM = 6     # gs3_cl_kernel: 40 registers, 18 KB of shared memory (emo_grid_sample3d)
 ACT_NAMES = ("none", "relu", "sigmoid", "tanh")
@@ -254,6 +256,21 @@ def classify(name: str, f: dict):
         if f["N"] * f["H"] * f["W"] > STRIDE_CAP * 256:
             feats.add("stem_pack grid-stride loop")
         return op, feats
+    if op == "pose_theta":
+        inp = "theta_in" if f["theta_in"] else "srt"
+        mix = ("mix_old" if f["mix_old"] else "mix") if f["mix"] else "nomix"
+        smooth = bool(f["smooth_state"])
+        cls = f"pose_theta {inp} {mix}{' smooth' if smooth else ''}"
+        inv = "invert" if f["invert_warp"] else "no invert"
+        feats |= {cls, f"pose {inp} {mix} {inv}", inv, "align" if f["align2d"] else "no align"}
+        if smooth:
+            start = "init" if f["smooth_init"] else "carried"
+            feats |= {f"smooth {start}", f"momentum {f['smooth_momentum']:.6g} {start}"}
+            if f["N"] > 1:
+                feats.add("one-thread walk")     # smoothing: one thread walks the samples in order
+        if f["N"] > 32:
+            feats.add("N > 32")                  # 32 threads per block
+        return cls, feats
     if op in BOUNDARY_GRID:
         # the wrapper-boundary kernels (tests/model_op_launches.py BOUNDARY): capped grid-stride loops
         work = {"u8_to_image": ("N", "H", "W"), "image_to_u8": ("N", "H", "W"), "composite": ("N", "C", "H", "W"),
@@ -401,11 +418,54 @@ CASES += [
 ]
 
 
-# C-ABI entry points outside the table: the convolution (tests/conv_plan_cases.py), the pose algebra
-# (tests/test_pose_math_host.py), the wrapper-boundary image conversions and mask kernels (tests/test_ops_gpu.py,
-# tests/test_masks.py, and at the wrappers' shapes the BOUNDARY launches of tests/model_op_launches.py) and the benchmark's
-# L2 flush
-NOT_IN_TABLE = ("conv_igemm", "pose_theta", "u8_to_image", "image_to_u8", "resize_bicubic", "composite", "parsing_prepare",
+def _pose(want, src, mix, invert, align, N, angles="inside", smooth=None, init=False):
+    """an emo_pose_theta case: src "srt" (angles "inside" the [-pi/2, pi] clamp, "beyond" it, or at its "edges") or
+    "theta_in" (a sheared affine); with smooth (the momentum), a call that seeds the state (init) or carries a seeded one"""
+    kw = dict(src=src, mix=mix, invert=invert, align=align, N=N, angles=angles if src == "srt" else "none")
+    if smooth is not None:
+        kw.update(smooth=smooth, init=init)
+    return case("pose_theta", want, **kw)
+
+
+CASES += [
+    # ---- emo_pose_theta: input x mix x invert, align2d set and NULL, one block and several ----
+    _pose("pose_theta srt nomix", "srt", "nomix", True, True, 1),
+    _pose("pose_theta srt nomix", "srt", "nomix", False, False, 32, "beyond"),
+    _pose("pose_theta srt mix", "srt", "mix", True, False, 33, "edges"),
+    _pose("pose_theta srt mix", "srt", "mix", False, True, 300),
+    _pose("pose_theta srt mix_old", "srt", "mix_old", True, True, 1, "beyond"),
+    _pose("pose_theta srt mix_old", "srt", "mix_old", False, False, 33, "edges"),
+    _pose("pose_theta theta_in nomix", "theta_in", "nomix", True, False, 300),
+    _pose("pose_theta theta_in nomix", "theta_in", "nomix", False, True, 1),
+    _pose("pose_theta theta_in mix", "theta_in", "mix", True, True, 32),
+    _pose("pose_theta theta_in mix", "theta_in", "mix", False, False, 33),
+    _pose("pose_theta theta_in mix_old", "theta_in", "mix_old", True, False, 1),
+    _pose("pose_theta theta_in mix_old", "theta_in", "mix_old", False, True, 300, "beyond"),
+    # smoothing: per momentum a call that seeds the state and one that carries a seeded state
+    _pose("pose_theta srt mix smooth", "srt", "mix", False, True, 3, smooth=0.5, init=True),
+    _pose("pose_theta srt mix smooth", "srt", "mix", True, False, 33, smooth=0.5),
+    _pose("pose_theta theta_in nomix smooth", "theta_in", "nomix", False, True, 1, smooth=0.3, init=True),
+    _pose("pose_theta theta_in nomix smooth", "theta_in", "nomix", False, False, 33, smooth=0.3),
+    _pose("pose_theta srt mix_old smooth", "srt", "mix_old", True, True, 4, smooth=0.9, init=True),
+    _pose("pose_theta theta_in nomix smooth", "theta_in", "nomix", False, True, 5, smooth=0.9),
+    _pose("pose_theta theta_in mix smooth", "theta_in", "mix", False, False, 2, smooth=0.6, init=True),
+    _pose("pose_theta srt nomix smooth", "srt", "nomix", True, True, 300, "beyond", smooth=0.6),
+    _pose("pose_theta srt nomix smooth", "srt", "nomix", False, True, 3, "beyond", smooth=0.99, init=True),
+    _pose("pose_theta theta_in mix_old smooth", "theta_in", "mix_old", False, True, 33, smooth=0.99),
+    _pose("pose_theta theta_in mix_old smooth", "theta_in", "mix_old", True, True, 5, smooth=0.01, init=True),
+    _pose("pose_theta srt mix smooth", "srt", "mix", False, False, 300, smooth=0.01),
+    _pose("pose_theta srt nomix smooth", "srt", "nomix", True, False, 2, smooth=0.0, init=True),
+    _pose("pose_theta theta_in mix smooth", "theta_in", "mix", True, True, 32, smooth=0.0),
+    _pose("pose_theta theta_in nomix smooth", "theta_in", "nomix", False, True, 3, smooth=1.0, init=True),
+    _pose("pose_theta srt mix_old smooth", "srt", "mix_old", False, False, 2, "edges", smooth=1.0),
+]
+POSE_MOMENTA = (0.5, 0.3, 0.9, 0.6, 0.99, 0.01, 0.0, 1.0)
+
+
+# C-ABI entry points outside the table: the convolution (tests/conv_plan_cases.py), the wrapper-boundary image conversions
+# and mask kernels (tests/test_ops_gpu.py, tests/test_masks.py, and at the wrappers' shapes the BOUNDARY launches of
+# tests/model_op_launches.py) and the benchmark's L2 flush
+NOT_IN_TABLE = ("conv_igemm", "u8_to_image", "image_to_u8", "resize_bicubic", "composite", "parsing_prepare",
                 "parsing_masks", "resize_area", "l2_flush", "l2_flush_clean")
 
 
@@ -419,6 +479,9 @@ def tags(c: Case) -> set:
         t.add("all-negative input")
     if c.op == "grid_sample2d_affine":
         t.add("lattice partly outside")
+    if c.op == "pose_theta":
+        t.add({"inside": "angles inside the clamp", "beyond": "angles beyond the clamp", "edges": "angles at -pi/2 and pi",
+               "none": "sheared affine theta_in"}[k["angles"]])
     return t
 
 
@@ -449,6 +512,11 @@ def required() -> list:
     req += ["same size", "up", "down", "non-integer ratio", "C_pad > C zero fill", "mean/std", "lattice partly outside", "NCHW copy"]
     req += ["split_bf16 x2", "split_bf16 x3", "split_f16 x2", "split_f16 x1"]
     req += ["stem_pack", "stem_pack grid-stride loop"]
+    pose = [(i, m) for i in ("srt", "theta_in") for m in ("nomix", "mix", "mix_old")]
+    req += [f"pose {i} {m} {v}" for i, m in pose for v in ("invert", "no invert")] + [f"pose_theta {i} {m} smooth" for i, m in pose]
+    req += ["invert", "no invert", "align", "no align", "smooth init", "smooth carried", "N > 32", "one-thread walk"]
+    req += [f"momentum {m:g} {s}" for m in POSE_MOMENTA for s in ("init", "carried")]
+    req += ["angles inside the clamp", "angles beyond the clamp", "angles at -pi/2 and pi", "sheared affine theta_in"]
     return req
 
 
@@ -573,7 +641,58 @@ def inputs(c: Case, device) -> dict:
         x = torch.zeros(k["N"], 1, k["H"], k["W"], 4)
         x[..., :3] = (torch.randn(k["N"], 1, k["H"], k["W"], 3, generator=g) * 1.5).clamp(-2.2, 2.7)   # normalised RGB
         t["x"] = x
+    elif c.op == "pose_theta":
+        t.update(pose_inputs(c, g))
     return {n: (v.to(device) if isinstance(v, torch.Tensor) else v) for n, v in t.items()}
+
+
+# the clamp's edges (it compares against the fp32 pi), exactly and one fp32 step either side of each, and 0
+POSE_EDGES = [-PR.PI32 / 2, PR.PI32, math.nextafter(-PR.PI32 / 2, -4.0), math.nextafter(PR.PI32, 4.0),
+              math.nextafter(-PR.PI32 / 2, 0.0), math.nextafter(PR.PI32, 0.0), 0.0]
+
+
+def _srt(N, g, angles):
+    """(N, 9) fp32 (scale 0.6-1.4, yaw pitch roll, translation +-0.5): wider than the head-pose regressor's range"""
+    s = 0.6 + 0.8 * torch.rand(N, 3, generator=g, dtype=torch.float64)
+    tr = torch.rand(N, 3, generator=g, dtype=torch.float64) - 0.5
+    if angles == "inside":
+        r = -1.5 + 4.5 * torch.rand(N, 3, generator=g, dtype=torch.float64)
+    elif angles == "beyond":
+        r = -5.0 + 10.0 * torch.rand(N, 3, generator=g, dtype=torch.float64)
+        r[0] = torch.tensor([-2.5, 4.0, -3.0])                           # every axis clamped, on both sides when N > 1
+        r[-1] = torch.tensor([4.5, -2.0, 3.7])
+    else:
+        r = torch.tensor([[POSE_EDGES[(n + 3 * a) % len(POSE_EDGES)] for a in range(3)] for n in range(N)], dtype=torch.float64)
+    return torch.cat([s, r, tr], 1).float()
+
+
+def _sheared_affine(N, g):
+    """(N, 4, 4) fp32 rotation . (scale 0.6-1.4 + shear up to 0.15) with translation +-0.5, last row [0, 0, 0, 1]: the polar
+    factors of its 3x3 part are not a rotation and a diagonal"""
+    th = torch.zeros(N, 4, 4, dtype=torch.float64)
+    for n in range(N):
+        q, _ = torch.linalg.qr(torch.randn(3, 3, generator=g, dtype=torch.float64))
+        st = torch.diag(0.6 + 0.8 * torch.rand(3, generator=g, dtype=torch.float64))
+        st += torch.triu(0.3 * torch.rand(3, 3, generator=g, dtype=torch.float64) - 0.15, 1)
+        th[n, :3, :3] = q @ st
+        th[n, :3, 3] = torch.rand(3, generator=g, dtype=torch.float64) - 0.5
+    th[:, 3, 3] = 1.0
+    return th.float()
+
+
+def pose_inputs(c: Case, g) -> dict:
+    """srt or theta_in, the source pose of a mixing case (of the same kind) and the state a carried smoothing case starts from"""
+    k, t = c.k, {}
+    if k["src"] == "srt":
+        t["srt"] = _srt(k["N"], g, k["angles"])
+    else:
+        t["theta_in"] = _sheared_affine(k["N"], g)
+    if k["mix"] != "nomix":
+        t["source_theta"] = (torch.from_numpy(PR.srt_theta(_srt(1, g, "inside"))).float() if k["src"] == "srt"
+                             else _sheared_affine(1, g))[0].contiguous()
+    if "smooth" in k and not k["init"]:
+        t["state0"] = torch.from_numpy(PR.srt_theta(_srt(1, g, "inside"))[0, :3]).float().contiguous()
+    return t
 
 
 def out_specs(c: Case) -> dict:
@@ -630,6 +749,13 @@ def out_specs(c: Case) -> dict:
         return {"planes": ((k["planes"], k["n"]), torch.bfloat16 if c.op == "split_bf16" else torch.float16)}
     if c.op == "stem_pack":
         return {"out": ((k["N"], 1, k["H"], k["W"], 32), torch.float16)}
+    if c.op == "pose_theta":
+        o = {"theta_out": ((k["N"], 4, 4), torch.float32), "theta_warp": ((k["N"], 3, 4), torch.float32)}
+        if k["align"]:
+            o["align2d"] = ((k["N"], 2, 3), torch.float32)
+        if "smooth" in k:
+            o["smooth_state"] = ((3, 4), torch.float32)
+        return o
     raise KeyError(c.op)
 
 
@@ -708,6 +834,14 @@ def launch(c: Case, ops, t: dict, o: dict):
         return name, (p(t["x"]), k["n"], C.c_float(F16_SCALE), pp[0], pp[1], ops._stream())
     if c.op == "stem_pack":
         return name, (p(t["x"]), k["N"], k["H"], k["W"], 4, C.c_float(F16_SCALE), p(o["out"]), ops._stream())
+    if c.op == "pose_theta":
+        st = o.get("smooth_state")
+        if st is not None and not k["init"]:
+            st.copy_(t["state0"])            # smooth_state is read and written: a carried case starts from the seeded state
+        d = ops.pose_desc(k["N"], p(t.get("srt")), p(t.get("source_theta")), p(o["theta_out"]), p(o["theta_warp"]),
+                          p(o.get("align2d")), p(t.get("theta_in")), p(st), mix=k["mix"] != "nomix", invert_warp=k["invert"],
+                          mix_old=k["mix"] == "mix_old", smooth_init=k.get("init", False), smooth_momentum=k.get("smooth", 0.5))
+        return name, (C.byref(d), ops._stream())
     raise KeyError(c.op)
 
 

@@ -50,6 +50,9 @@ def test_pose_theta_guards(L):
     _refused(L, "emo_pose_theta", P(FAKE, None, 0, 0, 0, FAKE, FAKE, FAKE, None, 0, 0, None, 0.5), "N must be positive")
     _refused(L, "emo_pose_theta", P(FAKE, None, 1, 1, 0, FAKE, FAKE, FAKE, None, 0, 0, None, 0.5), "mix needs source_theta")
     _refused(L, "emo_pose_theta", P(FAKE, None, 1, 0, 0, FAKE, FAKE, FAKE, None, 0, 0, FAKE, 1.5), "smooth_momentum")
+    _refused(L, "emo_pose_theta", P(FAKE, None, 1, 0, 0, FAKE, FAKE, FAKE, None, 0, 0, FAKE, 0.5, -0.5), "smooth_one_minus must be in [0,1]")
+    # a factor that does not belong to the momentum (zero, the layout before the field, derives it from the momentum)
+    _refused(L, "emo_pose_theta", P(FAKE, None, 1, 0, 0, FAKE, FAKE, FAKE, None, 0, 0, FAKE, 0.9, 0.9), "smooth_one_minus must be 1 - smooth_momentum")
 
 
 def test_mask_processing_guards(L):

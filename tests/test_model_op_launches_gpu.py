@@ -19,6 +19,8 @@ model-sized poses for the 3-D sampler).  Every output and every operand plane st
     per-group |mean| / std is op_cases.GN_ASSERTED_RATIO; their statistics match float64, and their output normalised by
     the fused apply matches float64 F.group_norm of it.  An apply that consumes statistics gets them built in float64 from
     its input with the recorded G, count and eps;
+  * the pose algebra (regressor-range poses, the source pass's pose as the mixing source) is within the per-entry bars of
+    its float64 restatement (tests/pose_reference.py), reported as error / bar;
   * two runs give bit-identical outputs (outputs over 1 GiB are compared by per-sample sums of their bit patterns) and
     statistics equal to 1e-13 relative (DESIGN.md section 2.4).
 Samples 0 and N - 1 are compared in full at batch >= 16 (the whole batch is checked for NaN); every sample otherwise.
@@ -47,12 +49,14 @@ MASK_FLIP_BOUND = 1e-5        # parsing_masks vs float64: pixels outside the 1e-
 STATS_REPRO = 1e-13
 FULL_BATCH = 15               # batches of 16 and more compare samples 0 and N - 1 against float64
 BIG = 1 << 30                 # outputs over 1 GiB: the two runs are compared by per-sample fingerprints
-ROWS = [("model", r) for r in MOL.load()] + [("boundary", r) for r in MOL.BOUNDARY]
+# the pose algebra's launches joined the table after the others: numbered last, so that every other launch keeps its id
+ROWS = ([("model", r) for r in MOL.load() if r["op"] != "pose_theta"] + [("boundary", r) for r in MOL.BOUNDARY]
+        + [("model", r) for r in MOL.load() if r["op"] == "pose_theta"])
 _WORST, _SKIPPED, _T0 = {}, [], []
 
 DESC = {"apply": "ApplyDesc", "gn_finalize": "GnFinalizeDesc", "gn_head": "GnHeadDesc", "grid_sample3d": "GridSample3dDesc",
         "grid_sample2d_affine": "GridSample2dAffineDesc", "resize_bilinear": "ResizeBilinearDesc", "linear": "LinearDesc",
-        "upsample_trilinear": "ResampleDesc", "avgpool": "ResampleDesc", "conv_direct": "ConvDirectDesc"}
+        "upsample_trilinear": "ResampleDesc", "avgpool": "ResampleDesc", "conv_direct": "ConvDirectDesc", "pose_theta": "PoseDesc"}
 SIZE_KEYS = ("N", "D", "H", "W", "C", "S", "n", "Din", "Hin", "Win", "Dout", "Hout", "Wout", "Cout", "M", "K", "fd", "fh", "fw", "up")
 
 
@@ -143,6 +147,10 @@ def out_specs(op, a, ptrs) -> dict:
         if "labels" in ptrs:
             o["labels"] = ((a["N"], 1, a["Hout"], a["Wout"]), u8)
         return o
+    if op == "pose_theta":
+        assert "smooth_state" not in ptrs, "the models do not smooth (the wrapper's smoothing is covered by tests/op_cases.py)"
+        shapes = {"theta_out": (a["N"], 4, 4), "theta_warp": (a["N"], 3, 4), "align2d": (a["N"], 2, 3)}
+        return {k: (s, f32) for k, s in shapes.items() if k in ptrs}
     raise KeyError(op)
 
 
@@ -168,6 +176,12 @@ def _pose_theta(N, g):
         th[n, :, :3] = R * s
         th[n, :, 3] = 0.4 * torch.rand(3, generator=gc, dtype=torch.float64) - 0.2
     return th.float().cuda()
+
+
+def _regressed_srt(N, g):
+    """(N, 9) head-pose regressor output of a face: scale 0.8-1.2, yaw / pitch / roll within +-0.8, translation +-0.2"""
+    u = torch.rand(N, 9, generator=g, device="cuda")
+    return torch.cat([0.8 + 0.4 * u[:, :3], 1.6 * u[:, 3:6] - 0.8, 0.4 * u[:, 6:] - 0.2], 1).contiguous()
 
 
 def _image(shape, g, lo=0.0, hi=1.0):
@@ -297,6 +311,15 @@ def inputs(op, a, ptrs, g) -> dict:
         t["img"], t["mask"], t["bg"] = _image((N, C_, H, W), g), _image((N, 1, H, W), g), _image((1, C_, H, W), g)[0]
     elif op == "parsing_masks":
         t["x"] = torch.randn((a["N"], a["K"], a["Hin"], a["Win"]), generator=g, device="cuda")    # white-noise logits
+    elif op == "pose_theta":
+        import pose_reference as PR
+
+        if "srt" in ptrs:
+            t["srt"] = _regressed_srt(a["N"], g)
+        if "theta_in" in ptrs:
+            t["theta_in"] = torch.from_numpy(PR.srt_theta(_regressed_srt(a["N"], g).cpu())).float().cuda()
+        if "source_theta" in ptrs:     # the source pass's pose
+            t["source_theta"] = torch.from_numpy(PR.srt_theta(_regressed_srt(1, g).cpu())[0]).float().cuda()
     else:
         raise KeyError(op)
     assert set(t) == set(ptrs) - set(out_specs(op, a, ptrs)), (op, sorted(t), ptrs)
@@ -485,7 +508,7 @@ def test_model_op_launch_against_float64(env, i):
     # ---- against float64 ----
     msg = f"\n[{cid}] {r['cls']}:"
     worst = _check(op, a, ptrs, t, o, samples, N, ops)
-    msg += f" error / scale {worst:.2e}"
+    msg += f" error / {'bar' if op == 'pose_theta' else 'scale'} {worst:.2e}"
     if stats_out:
         worst_gn, ratio = _check_groupnorm(op, a, o, t, samples, ops)
         msg += f"; GroupNorm mean/std {ratio:.1f}: normalised-output error {worst_gn:.2e}"
@@ -531,6 +554,11 @@ def _check(op, a, ptrs, t, o, samples, N, ops):
         return max(_cmp(o["A"], ref["A"], scale, "A"), _cmp(o["B"], ref["B"], scale, "B"))
     if op == "global_avgpool":
         return _cmp(o["out"], t["x"].double().mean(1), t["x"].abs().max().item(), "out")
+    if op == "pose_theta":      # every output within its float64 bar (tests/pose_reference.py): error / bar
+        import pose_reference as PR
+
+        mix = ("mix_old" if a["mix_old"] else "mix") if a["mix"] else "nomix"
+        return max(PR.check_outputs(t, o, mix, bool(a["invert_warp"])).values())
     for n in samples:
         ts = _sample(t, n, N)
         if op == "apply":

@@ -1,5 +1,6 @@
 """GPU sweep of the non-convolution kernels: every case of tests/op_cases.py (one per kernel variant, see
-tests/test_op_cases_cpu.py) against a float64 torch reference of the same op, and the GroupNorm edge cases.
+tests/test_op_cases_cpu.py) against a float64 torch reference of the same op, and the GroupNorm edge cases.  The pose
+algebra is held to the per-entry bars of its float64 restatement, tests/pose_reference.py.
 
 Per case: every output starts as NaN inside an allocation whose NaN tail is a guard region; after the call every element of the
 output is written and the guard is untouched.  Outputs match float64 within 2e-5 of their scale (the largest value the kernel
@@ -205,6 +206,10 @@ def reference(c, t):
         import test_fast_stage2_gpu as TS
 
         return {"plane": TS._stem_im2col(t["x"], OC.F16_SCALE)}, 1.0
+    if c.op == "pose_theta":     # (restatement, per-entry bars) of tests/pose_reference.py instead of (reference, scale)
+        import pose_reference as PR
+
+        return PR.pose64_of(t, k["mix"], k.get("smooth"), k.get("init", False), t.get("state0"))
     raise KeyError(c.op)
 
 
@@ -226,10 +231,18 @@ def test_op_case_against_float64(ops, c):
     for name, guard in guards.items():
         intact = (guard == STATS_GUARD).all() if name == "stats" else torch.isnan(guard.float()).all()
         assert intact, f"{name}: write past the end of the output (or of one of its planes)"
-    ref, scale = reference(c, t)
-    bound = TOL * max(1.0, scale)
     k = c.k
     msg = f"\n[{c.id}] {c.want}:"
+    if c.op == "pose_theta":     # per-entry float64 bars instead of one scale
+        import pose_reference as PR
+
+        ref, bar = reference(c, t)
+        e = PR.compare(o, ref, bar, k["invert"])
+        _note("pose_theta (error / bar)", max(e.values()), c.id)
+        print(msg + "".join(f" {n} {v:.2f} of its bar" for n, v in e.items()))
+        return
+    ref, scale = reference(c, t)
+    bound = TOL * max(1.0, scale)
     kernel = c.want.split(" ")[0] if not c.op.startswith("split") else c.op
     exact = (c.op == "maxpool2d_3x3s2" or c.op.startswith("split")
              or (c.op in ("upsample_trilinear", "avgpool") and k["f"] == (1, 1, 1) and not k["add"])
@@ -297,7 +310,7 @@ def test_op_case_against_float64(ops, c):
 
 
 def test_report_largest_error_per_kernel():
-    """(runs after the sweep) the largest error / max(1, scale) seen per kernel"""
+    """(runs after the sweep) the largest error / max(1, scale) seen per kernel (pose_theta: error / its float64 bar)"""
     if not _WORST:
         pytest.skip("no sweep case ran")
     for k, (rel, cid) in sorted(_WORST.items()):

@@ -385,6 +385,7 @@ def test_maxpool_and_global_avgpool(ops):
 
 
 def test_pose_theta(ops):
+    """smoke test of ops.pose_theta against the oracle; tests/test_pose_kernel_gpu.py checks the kernel in every mode"""
     from oracle import restatement as R
     srt = torch.tensor([[1.0, 1.1, 0.9, 0.15, -0.1, 0.05, 0.03, -0.02, 0.01], [0.8, 0.9, 1.0, -0.3, 0.2, 0.1, -0.1, 0.05, 0.0]])
     th_ref = R.get_transform_matrix(srt[:, :3], srt[:, 3:6], srt[:, 6:])

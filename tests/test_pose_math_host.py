@@ -2,11 +2,10 @@
 CUDA kernel pose_theta_kernel calls pose::pose_sample() per sample; here the same file is compiled with g++ and driven
 through the same emo_pose_desc (ctypes structure of emoportraits_b200/lib.py) with HOST pointers, and compared with
 the oracle (oracle/restatement.py: torch + scipy.linalg.polar, as the reference computes it) and with the poses the
-unmodified reference produced (tests/golden/va256_options.pt).  This is test infrastructure: the product never calls
+unmodified reference produced (tests/golden/va256_options.pt).  The build itself is tests/pose_reference.host_build, which
+tests/test_pose_kernel_gpu.py compares the device build with.  This is test infrastructure: the product never calls
 the host build (the GPU parity tests call the kernel through the C-ABI)."""
-import ctypes as C
 import pathlib
-import subprocess
 
 import numpy as np
 import pytest
@@ -15,41 +14,12 @@ import torch
 ROOT = pathlib.Path(__file__).resolve().parents[1]
 GOLD = ROOT / "tests" / "golden"
 
-SHIM = r'''
-#include "emoportraits_b200/csrc/pose_math.cuh"
-extern "C" void pose_host(const emo_pose_desc* d) {
-  for (int n = 0; n < d->N; ++n) emo::pose::pose_sample(*d, n);
-}
-'''
-
 
 @pytest.fixture(scope="module")
 def host(tmp_path_factory):
-    d = tmp_path_factory.mktemp("pose_host")
-    (d / "shim.cpp").write_text(SHIM)
-    so = d / "libpose_host.so"
-    subprocess.run(["g++", "-O2", "-ffp-contract=off", "-std=c++17", "-shared", "-fPIC", "-I", str(ROOT), "-x", "c++",
-                    str(d / "shim.cpp"), "-o", str(so)], check=True)
-    lib = C.CDLL(str(so))
-    from emoportraits_b200.lib import PoseDesc
+    import pose_reference as PR
 
-    lib.pose_host.argtypes = [C.POINTER(PoseDesc)]
-    lib.pose_host.restype = None
-
-    def run(srt=None, source_theta=None, mix=False, invert_warp=False, mix_old=False, theta_in=None, smooth_state=None,
-            smooth_momentum=0.5, smooth_init=False):
-        ref = srt if srt is not None else theta_in
-        N = ref.shape[0]
-        f = lambda a: None if a is None else np.ascontiguousarray(a, dtype=np.float32)
-        srt, source_theta, theta_in = f(srt), f(source_theta), f(theta_in)
-        theta, warp, align = (np.zeros((N, 4, 4), np.float32), np.zeros((N, 3, 4), np.float32), np.zeros((N, 2, 3), np.float32))
-        p = lambda a: None if a is None else a.ctypes.data
-        desc = PoseDesc(p(srt), p(source_theta), N, int(mix), int(invert_warp), p(theta), p(warp), p(align), p(theta_in),
-                        int(mix_old), int(smooth_init), p(smooth_state), float(smooth_momentum))
-        lib.pose_host(C.byref(desc))
-        return torch.from_numpy(theta), torch.from_numpy(warp), torch.from_numpy(align)
-
-    return run
+    return PR.host_build(tmp_path_factory.mktemp("pose_host"))
 
 
 def _srt(n, seed, wild=False):
@@ -92,7 +62,7 @@ def test_mixing_matches_scipy_polar(host, mix_old):
     assert (theta2 - theta).abs().max().item() < 1e-6
 
 
-@pytest.mark.parametrize("momentum", [0.5, 0.3])
+@pytest.mark.parametrize("momentum", [0.5, 0.3, 0.9, 0.6, 0.99])
 def test_smoothing_is_the_reference_recurrence_bit_for_bit(host, momentum):
     from oracle import restatement as R
 
