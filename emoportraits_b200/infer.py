@@ -147,7 +147,7 @@ class Model:
                     want_logits: bool = False, pose_override=None, mix_old: bool = False,
                     custom_srt: Optional[torch.Tensor] = None, custom_pose_embed: Optional[torch.Tensor] = None,
                     smooth_state: Optional[torch.Tensor] = None, smooth_momentum: float = 0.5, smooth_init: bool = False,
-                    encode_only: bool = False):
+                    encode_only: bool = False, pose_only: bool = False, pose_in: Optional[tuple] = None):
         """drv (1,3,H,W) fp32 on device -> (img (1,3,H,W), feat_2d, img_feat, state).
         mix / mix_old: get_mixing_theta (infer.py:569-570, 686-736).  custom_srt (1,9) = the caller's
         custome_target_theta_embed (scale, rotation, translation) replacing the regressed pose (:566-567).
@@ -156,22 +156,36 @@ class Model:
         drv=None (both custom_srt and custom_pose_embed given): an image-free frame, without the head-pose regressor and the
         expression encoder; state.srt is then custom_srt.  encode_only: stop after the expression encoder and return
         (None, None, None, state): the frame's regressed pose state.srt and its embedding state.target_pose_embed, whose 2-D
-        alignment comes from the mixed pose (so it depends on mix / mix_old and, with mix, on st's source pose)."""
+        alignment comes from the mixed pose (so it depends on mix / mix_old and, with mix, on st's source pose).
+        A smoothing frame in flight (DriverPipeline(smooth=True)) runs in two parts around its pose step, the one launch that
+        carries state from frame to frame.  pose_only: stop after the pose algebra and return (None, None, None, state) with
+        state.pred_target_theta the (1,4,4) pose, mixed and not smoothed, and state.srt.  pose_in = (theta (1,4,4), warp
+        (1,3,4), align (1,2,3)): the pose step already wrote the frame's pose there; skip the head-pose regressor and the pose
+        algebra and run the rest of the frame on it (state.srt is then None)."""
         cfg = self.cfg
-        if drv is None and (custom_srt is None or custom_pose_embed is None or encode_only or taps is not None):
+        if drv is None and (custom_pose_embed is None or (custom_srt is None and pose_in is None) or encode_only
+                            or taps is not None):
             raise ValueError("driver_pass: a frame without a driver image needs custom_srt and custom_pose_embed")
+        if pose_in is not None and (pose_only or smooth_state is not None or pose_override is not None):
+            raise ValueError("driver_pass: pose_in is the frame's finished pose; it takes no pose_only, smoothing or override")
         if drv is not None:
             drv = drv.contiguous().float()
         ops.begin_pass(self.device)
-        srt = None if drv is None else self.head_pose_regressor(drv)
-        srt_used = srt if custom_srt is None else custom_srt.to(self.device).float().reshape(1, 9).contiguous()
-        if srt is None:
-            srt = srt_used     # an image-free frame reports the supplied pose
-        theta, warp, align = ops.pose_theta(srt_used, source_theta=st.source_theta_dev if mix else None, mix=mix,
-                                            mix_old=mix_old, smooth_state=smooth_state, smooth_momentum=smooth_momentum,
-                                            smooth_init=smooth_init)
+        if pose_in is not None:
+            srt = None
+            theta, warp, align = pose_in
+        else:
+            srt = None if drv is None else self.head_pose_regressor(drv)
+            srt_used = srt if custom_srt is None else custom_srt.to(self.device).float().reshape(1, 9).contiguous()
+            if srt is None:
+                srt = srt_used     # an image-free frame reports the supplied pose
+            theta, warp, align = ops.pose_theta(srt_used, source_theta=st.source_theta_dev if mix else None, mix=mix,
+                                                mix_old=mix_old, smooth_state=smooth_state, smooth_momentum=smooth_momentum,
+                                                smooth_init=smooth_init)
         if pose_override is not None:
             theta, warp, align = [t.to(self.device).float().contiguous() for t in pose_override]
+        if pose_only:
+            return None, None, None, SimpleNamespace(pred_target_theta=theta, target_pose_embed=None, srt=srt)
         if custom_pose_embed is not None and taps is None:
             pose_embed, aligned = None, None      # the expression encoder's output would be discarded (infer.py:602-603)
         else:
@@ -241,7 +255,7 @@ class Model:
     def make_driver_graph(self, st, mix: bool = True, target_theta: bool = True, slot: int = 0, mix_old: bool = False,
                           smooth_state: Optional[torch.Tensor] = None, smooth_momentum: float = 0.5, image: bool = True,
                           theta_embed: bool = False, pose_embed: bool = False, encode: bool = False, refine=None,
-                          refine_masks: Optional[dict] = None, composite=None):
+                          refine_masks: Optional[dict] = None, composite=None, pose_step: bool = False):
         """Capture one driver frame (all ~240 kernel launches) into a CUDA graph: removes the Python/ctypes launch
         overhead from the per-frame loop.  Returns replay(drv (1,3,H,W) on device) -> img (1,3,H,W) (static buffer).
         The graph reads its identity from buffers of its own (replay.identity, dist.new_identity), never from `st`:
@@ -268,19 +282,41 @@ class Model:
         which the caller fills before a replay, as video.connect_img_and_bg does, before stage 2.  The caller's networks are
         captured with the frame (INTEGRATION.md "Mask networks in captured frames": no host syncs, static shapes, already on
         this device); the warm-up passes run them too.  A capture that fails raises RuntimeError naming the network that
-        broke it."""
+        broke it.
+        pose_step: the frame is captured as two graphs around its pose step, for frames whose poses are smoothed in flight
+        (DriverPipeline(smooth=True)).  replay.head_graph runs the input side up to the pose algebra, mixed but not smoothed,
+        into replay.static_mixed (1,4,4); the caller then runs Model.pose_step from it into replay.pose (theta (1,4,4), warp
+        (1,3,4), align (1,2,3)), and replay.graph runs the rest of the frame from there.  Not with smooth_state or encode."""
         self.check_inputs(image, theta_embed, pose_embed, encode)
         self.check_refine(refine, encode)
         self.check_refine_masks(refine, refine_masks, composite)
+        self.check_pose_step(pose_step, encode, smooth_state)
         prev = ops.set_slot(slot)
         try:
             return self._make_driver_graph(st, mix, target_theta, mix_old, smooth_state, smooth_momentum, image, theta_embed,
-                                           pose_embed, encode, refine, refine_masks, composite)
+                                           pose_embed, encode, refine, refine_masks, composite, pose_step)
         finally:
             ops.set_slot(prev)
 
+    @staticmethod
+    def check_pose_step(pose_step: bool, encode: bool, smooth_state=None) -> None:
+        """ValueError unless a frame split at its pose step (make_driver_graph(pose_step=True)) can take these options"""
+        if pose_step and encode:
+            raise ValueError("smoothing frames in flight render their frames: smooth needs encode=False")
+        if pose_step and smooth_state is not None:
+            raise ValueError("a frame split at its pose step is smoothed by the pose step, not in the graph: no smooth_state")
+
+    @staticmethod
+    def pose_step(mixed: torch.Tensor, state: torch.Tensor, momentum: float, init: bool, out: tuple):
+        """The pose step of a smoothing frame in flight, between its two graphs: smooths the frame's mixed pose (1,4,4) into
+        the (3,4) state in place (seeding it first if init, the reference's `self.theta is None`), and writes the smoothed
+        pose, its warp and 2-D alignment into `out`.  driver_pass's pose algebra keeps the mixed pose in fp32 and rereads
+        it here unchanged, so this launch smooths, inverts and aligns exactly what one smoothing launch would."""
+        return ops.pose_theta(None, theta_in=mixed, smooth_state=state, smooth_momentum=momentum, smooth_init=init, out=out)
+
     def _make_driver_graph(self, st, mix, target_theta, mix_old=False, smooth_state=None, smooth_momentum=0.5, image=True,
-                           theta_embed=False, pose_embed=False, encode=False, refine=None, refine_masks=None, composite=None):
+                           theta_embed=False, pose_embed=False, encode=False, refine=None, refine_masks=None, composite=None,
+                           pose_step=False):
         s, dev = self.cfg.image_size, self.device
         static_in = torch.zeros((1, 3, s, s), dtype=torch.float32, device=dev) if image else None
         # the warm-up passes run on the unit pose (scale 1, no rotation or translation) and a zero embedding
@@ -293,8 +329,15 @@ class Model:
         if smooth_state is not None:
             kw.update(smooth_state=smooth_state, smooth_momentum=smooth_momentum, smooth_init=False)
             saved = smooth_state.clone()  # the warm-up and capture passes smooth a dummy frame into the state: put it back after
+        # a frame split at its pose step: the pose buffers the step writes and the tail reads, and a state for the warm-up
+        pose = tuple(torch.zeros(shp, dtype=torch.float32, device=dev) for shp in ((1, 4, 4), (1, 3, 4), (1, 2, 3))) \
+            if pose_step else None
+        warm_state = torch.zeros((3, 4), dtype=torch.float32, device=dev) if pose_step else None
+        head_graph = head = None
 
         def replay(drv: torch.Tensor) -> torch.Tensor:
+            if head_graph is not None:
+                raise RuntimeError("a frame split at its pose step runs through DriverPipeline(smooth=True).submit(..., track=)")
             static_in.copy_(drv, non_blocking=True)
             graph.replay()
             return static_out
@@ -333,19 +376,30 @@ class Model:
                 return refine.refine(img, matte=matte, bg=static_bg, **{k: v for k, v in refine_kw.items() if k != "composite"})
             return refine.refine(img, **refine_kw)
 
+        def warm_frame():
+            if not pose_step:
+                return self.driver_pass(identity, static_in, **kw)[0]
+            mixed = self.driver_pass(identity, static_in, pose_only=True, **kw)[3].pred_target_theta
+            self.pose_step(mixed, warm_state, 0.5, True, pose)
+            return self.driver_pass(identity, static_in, pose_in=pose, **kw)[0]
+
         side = torch.cuda.Stream(device=self.device)
         side.wait_stream(torch.cuda.current_stream(self.device))
         try:
             with torch.cuda.stream(side):
                 for _ in range(2):
-                    img = self.driver_pass(identity, static_in, **kw)[0]
+                    img = warm_frame()
                     if refine is not None:
                         refined(img)
             torch.cuda.current_stream(self.device).wait_stream(side)
             torch.cuda.synchronize(self.device)
+            if pose_step:
+                head_graph = torch.cuda.CUDAGraph()
+                with torch.cuda.graph(head_graph):
+                    head = self.driver_pass(identity, static_in, pose_only=True, **kw)[3]
             graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(graph):
-                out = self.driver_pass(identity, static_in, **kw)
+                out = self.driver_pass(identity, static_in, pose_in=pose, **kw)
                 static_out = static_stage1 = out[0]
                 static_u8 = None
                 if refine is not None:
@@ -360,8 +414,12 @@ class Model:
         if smooth_state is not None:
             smooth_state.copy_(saved)
 
-        replay.graph = graph
-        replay.static_in, replay.static_out, replay.static_state = static_in, static_out, out[3]
+        so = out[3]
+        if pose_step:    # the frame's regressed (or supplied) pose comes from its head
+            so = SimpleNamespace(pred_target_theta=so.pred_target_theta, target_pose_embed=so.target_pose_embed, srt=head.srt)
+        replay.graph, replay.head_graph = graph, head_graph
+        replay.static_mixed, replay.pose = (head.pred_target_theta if pose_step else None), pose
+        replay.static_in, replay.static_out, replay.static_state = static_in, static_out, so
         replay.static_theta, replay.static_pose = static_theta, static_pose
         replay.static_stage1, replay.static_u8, replay.static_bg = static_stage1, static_u8, static_bg
         return replay
@@ -390,6 +448,31 @@ def _named_networks(refine_masks: dict, composite, culprit: list) -> dict:
     return out
 
 
+class PoseTrack:
+    """The pose-smoothing state of one stream of driver frames (one webcam, one participant of a call): the (3,4) fp32 state
+    on the device (the reference wrapper's self.theta), the momentum it is smoothed with (theta * m + state * (1 - m),
+    notebooks/infer.py:571-581), whether it is seeded, and the event of its last pose step.  Made by DriverPipeline.track;
+    the first frame after creation or reset() seeds the state with its own pose.  momentum may be changed between frames:
+    it is an argument of each pose step, not part of a captured graph."""
+
+    def __init__(self, device, momentum: float = 0.5, state: Optional[torch.Tensor] = None):
+        self.momentum = self.check_momentum(momentum)
+        self.state = torch.zeros((3, 4), dtype=torch.float32, device=device) if state is None else state
+        self.seeded = False
+        self.event = None   # recorded after the track's last pose step; the next one waits for it
+
+    @staticmethod
+    def check_momentum(momentum) -> float:
+        m = float(momentum)
+        if not 0.0 <= m <= 1.0:
+            raise ValueError(f"pose momentum must be in [0, 1], got {momentum!r}")
+        return m
+
+    def reset(self) -> None:
+        """the next frame seeds the state (reset_tracking)"""
+        self.seeded = False
+
+
 class DriverPipeline:
     """Keeps `depth` driver frames in flight on one GPU.  Driver frames are independent given the cached source state
     (notebooks/infer.py:511-644 reads only self.* source tensors), and roughly a quarter of a frame is a chain of ~120
@@ -412,25 +495,40 @@ class DriverPipeline:
     slot.run.static_out is the refined (1,3,S2,S2) image, slot.run.static_u8 its uint8 frame and slot.run.static_stage1 the
     stage-1 image.  submit(..., u8_out=) copies the uint8 frame out on the frame's stream.
     refine_masks / composite: stage 2's mask networks and the compositing matte network (Model.make_driver_graph), captured
-    with every frame; a compositing pipeline's frames take submit(..., bg=)."""
+    with every frame; a compositing pipeline's frames take submit(..., bg=).
+
+    smooth: every frame's pose is smoothed over the frames of its track (smooth_pose, notebooks/infer.py:571-581), with the
+    frames still in flight.  Only one launch of a frame carries state from frame to frame, so each slot captures its frame
+    as two graphs around it (Model.make_driver_graph(pose_step=True)); between them the frame's pose step
+    (Model.pose_step) runs on the pipeline's pose stream, after the frame's head and after its track's previous pose step.
+    submit order is the order of each track's recurrence.  Every frame names its track: submit(..., track=pipe.track()),
+    one PoseTrack per incoming stream of frames."""
 
     def __init__(self, model: "Model", st, depth: int = 2, mix: bool = True, target_theta: bool = True, mix_old: bool = False,
                  image: bool = True, theta_embed: bool = False, pose_embed: bool = False, encode: bool = False, refine=None,
-                 refine_masks: Optional[dict] = None, composite=None):
+                 refine_masks: Optional[dict] = None, composite=None, smooth: bool = False):
         model.check_inputs(image, theta_embed, pose_embed, encode)
         model.check_refine(refine, encode)
         Model.check_refine_masks(refine, refine_masks, composite)
+        Model.check_pose_step(smooth, encode)
         self.model, self.depth, self.n = model, depth, 0
         self.image, self.theta_embed, self.pose_embed, self.encode = image, theta_embed, pose_embed, encode
-        self.refine, self.composite = refine, composite
+        self.refine, self.composite, self.smooth = refine, composite, smooth
         self.st = st  # the current identity: frames submitted without st= animate it
+        # the pose steps of all the pipeline's frames, in submit order: only tiny launches run here
+        self.pose_stream = torch.cuda.Stream(device=model.device) if smooth else None
         self.slots = []
         for k in self.scratch_slots(depth):
             run = model.make_driver_graph(st, mix=mix, target_theta=target_theta, slot=k, mix_old=mix_old, image=image,
                                           theta_embed=theta_embed, pose_embed=pose_embed, encode=encode, refine=refine,
-                                          refine_masks=refine_masks, composite=composite)
+                                          refine_masks=refine_masks, composite=composite, pose_step=smooth)
             self.slots.append(SimpleNamespace(run=run, stream=torch.cuda.Stream(device=model.device),
                                               done=torch.cuda.Event(), busy=False, bg=None))
+
+    def track(self, momentum: float = 0.5) -> PoseTrack:
+        """a new pose track on this pipeline's device (a smoothing pipeline's frames name theirs in submit(..., track=)); it
+        may be used by several pipelines of the device, its frames then ordered by submit across them"""
+        return PoseTrack(self.model.device, momentum)
 
     @staticmethod
     def scratch_slots(depth: int) -> list:
@@ -438,9 +536,19 @@ class DriverPipeline:
         (Model.source_pass / driver_pass on the current stream), which may overlap frames in flight."""
         return [k + 1 for k in range(depth)]
 
-    def _check_submit(self, drv, theta_embed, pose_embed, outs, u8_out=None, bg=None) -> None:
+    def _check_submit(self, drv, theta_embed, pose_embed, outs, u8_out=None, bg=None, track=None) -> None:
         """ValueError unless a frame's inputs are the ones the pipeline was captured for, of the right shapes, u8_out
-        a (1,S2,S2,3) uint8 buffer of a refining pipeline and bg a (3,H,W) fp32 background of a compositing one"""
+        a (1,S2,S2,3) uint8 buffer of a refining pipeline, bg a (3,H,W) fp32 background of a compositing one and track a
+        PoseTrack on this device, given exactly when the pipeline smooths"""
+        if (track is not None) != bool(getattr(self, "smooth", False)):
+            raise ValueError("track= names the pose track of a frame of a smoothing pipeline (smooth=True): give it exactly when "
+                             "the pipeline smooths")
+        if track is not None:
+            if not isinstance(track, PoseTrack):
+                raise ValueError(f"track must be a PoseTrack (DriverPipeline.track()), got {type(track).__name__}")
+            if ops._dev_key(track.state.device) != ops._dev_key(self.model.device):
+                raise ValueError(f"the track's state is on {track.state.device}, the pipeline on {self.model.device}")
+            PoseTrack.check_momentum(track.momentum)
         if (bg is not None) != (getattr(self, "composite", None) is not None):
             raise ValueError("bg= is the background of a compositing pipeline (composite=): give it exactly when the pipeline "
                              "composites")
@@ -472,7 +580,7 @@ class DriverPipeline:
 
     def submit(self, drv: Optional[torch.Tensor], host_out: Optional[torch.Tensor] = None, dev_out: Optional[torch.Tensor] = None,
                st=None, theta_embed: Optional[torch.Tensor] = None, pose_embed: Optional[torch.Tensor] = None,
-               u8_out: Optional[torch.Tensor] = None, bg: Optional[torch.Tensor] = None):
+               u8_out: Optional[torch.Tensor] = None, bg: Optional[torch.Tensor] = None, track: Optional[PoseTrack] = None):
         """Queue one frame (device tensor, or pinned host tensor -> asynchronous H2D on the frame's stream).  If `host_out`
         (pinned) / `dev_out` is given the image is copied into it on the same stream.  Returns a ticket: ticket.done is an
         event recorded when this frame (and its copy-out) has finished (ticket.slot.done is the same event, i.e. always the
@@ -489,10 +597,13 @@ class DriverPipeline:
         (slot.run.static_u8) is copied into it on the frame's stream, before ticket.done.
         bg (3,H,W) fp32 (a compositing pipeline only, and then for every frame): the background the frame is composited over.  A
         slot copies it into its buffer (slot.run.static_bg) on its stream only when it is a different tensor from the slot's
-        last one; the slot keeps a reference to it and marks it as in use by its stream, as replay.load does an identity."""
+        last one; the slot keeps a reference to it and marks it as in use by its stream, as replay.load does an identity.
+        track (a smoothing pipeline only, and then for every frame): the PoseTrack whose state the frame's pose is smoothed
+        into.  The frame's pose step waits for its head and for the track's last pose step, on any pipeline; the state is
+        seeded by the track's first frame after creation or reset(), and smoothed with track.momentum as it is at submit."""
         if st is not None:
             check_identity(st, self.model.cfg)
-        self._check_submit(drv, theta_embed, pose_embed, (host_out, dev_out), u8_out, bg)
+        self._check_submit(drv, theta_embed, pose_embed, (host_out, dev_out), u8_out, bg, track)
         if st is not None:
             self.st = st
         sl = self.slots[self.n % self.depth]
@@ -510,6 +621,8 @@ class DriverPipeline:
                 sl.bg = bg
             for buf, t in inputs:
                 buf.copy_(t, non_blocking=True)
+            if track is not None:
+                self._pose_step(sl, track)
             sl.run.graph.replay()
             if host_out is not None:
                 host_out.copy_(sl.run.static_out, non_blocking=True)
@@ -521,6 +634,23 @@ class DriverPipeline:
             sl.done.record()
         sl.busy = True
         return SimpleNamespace(done=sl.done, slot=sl, index=self.n - 1)
+
+    def _pose_step(self, sl, track: PoseTrack) -> None:
+        """on the slot's stream: the frame's head, then (on the pose stream) its pose step, which the tail waits for"""
+        sl.run.head_graph.replay()
+        head = torch.cuda.Event()
+        head.record()
+        with torch.cuda.stream(self.pose_stream):
+            self.pose_stream.wait_event(head)
+            if track.event is not None:
+                self.pose_stream.wait_event(track.event)
+            if track.state.is_cuda:
+                track.state.record_stream(self.pose_stream)   # a caller may drop the track before its last step ran
+            Model.pose_step(sl.run.static_mixed, track.state, track.momentum, not track.seeded, sl.run.pose)
+            track.event = torch.cuda.Event()
+            track.event.record()
+        track.seeded = True
+        sl.stream.wait_event(track.event)
 
     def drain(self):
         cur = torch.cuda.current_stream(self.model.device)
@@ -592,6 +722,7 @@ class InferenceWrapper(torch.nn.Module):
         self._state = None
         self._pipelines = OrderedDict()   # captured DriverPipelines by options, least recently used first
         self._smooth_graph = None
+        self._track = None                # the PoseTrack of smoothed frames in flight: its state is self.theta
         # external mask networks (separate checkouts in the reference: repos/face_par_off behind model.face_idt, infer.py:410;
         # repos/MODNet, infer.py:140-149): None until the caller plugs them in (masks.FaceParsing(None, net=...), any MODNet module)
         self.face_idt = None
@@ -665,15 +796,36 @@ class InferenceWrapper(torch.nn.Module):
             self._pipelines.popitem(last=False)
         return pipe
 
-    def _forward_list(self, frames, mix, target_theta, mix_old, theta_embed=None, pose_embed=None):
+    def _forward_list(self, frames, mix, target_theta, mix_old, theta_embed=None, pose_embed=None, track=None):
         """A list of PIL / numpy driver frames: every frame is converted, uploaded and queued on its own (four captured frames in
         flight), its uint8 image is produced and copied back on the frame's stream, so the host-side conversions of frame i + 1
         overlap the device work of frame i; the PIL images are wrapped as their copies land.  Same results as one call per frame.
-        theta_embed (1,9) / pose_embed (1,E) on the device: the caller's pose / embedding for every frame."""
+        theta_embed (1,9) / pose_embed (1,E) on the device: the caller's pose / embedding for every frame.  track: the
+        frames' poses are smoothed into this PoseTrack (smooth_pose), through the smoothing pipeline."""
+        smooth = dict(smooth=True) if track is not None else {}
         pipe = self._driver_pipeline(mix, target_theta, mix_old, theta_embed=theta_embed is not None,
-                                     pose_embed=pose_embed is not None)
-        return self._render(pipe, len(frames), lambda i: dict(drv=self._prep(frames[i]), theta_embed=theta_embed,
-                                                              pose_embed=pose_embed))
+                                     pose_embed=pose_embed is not None, **smooth)
+        with_track = (lambda kw: dict(kw, track=track)) if track is not None else (lambda kw: kw)
+        return self._render(pipe, len(frames), lambda i: with_track(dict(drv=self._prep(frames[i]), theta_embed=theta_embed,
+                                                                         pose_embed=pose_embed)))
+
+    def _pose_track(self) -> PoseTrack:
+        """the wrapper's own pose track for smoothed frames in flight, with the wrapper's pose_momentum: its state tensor is
+        self.theta, which single smoothed frames carry on, and it is seeded unless tracking was reset (self.theta is None).
+        The captured single-frame graph smooths into the same tensor; forward drains the pipeline before it returns, so
+        the two paths never overlap."""
+        momentum = PoseTrack.check_momentum(self.pose_momentum)
+        init = self.theta is None
+        tr = self._track
+        if init:
+            g = self._smooth_graph
+            self.theta = g.theta if g is not None else tr.state if tr is not None else \
+                torch.zeros((3, 4), dtype=torch.float32, device=self.device)
+        if tr is None or tr.state is not self.theta:
+            tr = self._track = PoseTrack(self.device, momentum, state=self.theta)
+        tr.momentum = momentum
+        tr.seeded = not init
+        return tr
 
     def _render(self, pipe, n, inputs):
         """n frames through `pipe`, frame i with the submit arguments inputs(i), returned as forward returns them; sets the
@@ -954,17 +1106,25 @@ class InferenceWrapper(torch.nn.Module):
         embeds = dict(theta_embed=None if custom_srt is None else custom_srt.to(self.device).contiguous(),
                       pose_embed=None if custome_target_pose_embed is None else
                       torch.as_tensor(custome_target_pose_embed).to(self.device).float().reshape(1, -1).contiguous())
-        if not smooth_pose and isinstance(driver_image, list) and len(driver_image) > 1 and not isinstance(driver_image[0], torch.Tensor):
-            return self._forward_list(driver_image, mix, target_theta, mix_old, **embeds)
+        # smoothed frames, more than one, with the regressed pose and embedding: in flight too, smoothed by the pose steps of
+        # the wrapper's track (DriverPipeline(smooth=True)).  A single smoothed frame keeps its one captured graph below
+        smooth_custom = smooth_pose and (custom_srt is not None or custome_target_pose_embed is not None)
+        if not smooth_custom and isinstance(driver_image, list) and len(driver_image) > 1 and \
+                not isinstance(driver_image[0], torch.Tensor):
+            track = self._pose_track() if smooth_pose else None
+            return self._forward_list(driver_image, mix, target_theta, mix_old, **embeds, track=track)
         drv = self._prep(driver_image)
-        if not smooth_pose:
+        if not smooth_pose or (not smooth_custom and drv.shape[0] > 1):
             # captured driver frames (CUDA graphs), four in flight when a list of frames is given (DriverPipeline); same
             # kernels as the eager pass below.  With a custom pose / embedding the graphs take it as an input; the
             # expression encoder is then not captured, and pred_target_srt stays the regressed pose (infer.py:563-564)
-            pipe = self._driver_pipeline(mix, target_theta, mix_old, **{k: v is not None for k, v in embeds.items()})
+            track = self._pose_track() if smooth_pose else None
+            smooth = dict(smooth=True) if track is not None else {}
+            with_track = dict(track=track) if track is not None else {}
+            pipe = self._driver_pipeline(mix, target_theta, mix_old, **{k: v is not None for k, v in embeds.items()}, **smooth)
             img = torch.empty_like(drv)
             for i in range(drv.shape[0]):
-                sl = pipe.submit(drv[i:i + 1], dev_out=img[i:i + 1], st=self._state, **embeds).slot
+                sl = pipe.submit(drv[i:i + 1], dev_out=img[i:i + 1], st=self._state, **embeds, **with_track).slot
             pipe.drain()
             so = sl.run.static_state
             self.pred_target_theta = so.pred_target_theta.clone()

@@ -644,9 +644,11 @@ def global_avgpool(x: torch.Tensor):
 
 def pose_theta(srt: Optional[torch.Tensor], source_theta: Optional[torch.Tensor] = None, mix: bool = False,
                invert_warp: bool = False, mix_old: bool = False, theta_in: Optional[torch.Tensor] = None,
-               smooth_state: Optional[torch.Tensor] = None, smooth_momentum: float = 0.5, smooth_init: bool = False):
+               smooth_state: Optional[torch.Tensor] = None, smooth_momentum: float = 0.5, smooth_init: bool = False,
+               out: Optional[tuple] = None):
     """srt (N,9) [or theta_in (N,4,4)] -> theta (N,4,4), theta_warp (N,3,4), align2d (N,2,3). See emo_pose_theta.
-    smooth_state (3,4) fp32 on device is updated in place (smooth_pose=True, notebooks/infer.py:571-581)."""
+    smooth_state (3,4) fp32 on device is updated in place (smooth_pose=True, notebooks/infer.py:571-581).
+    out: (theta, theta_warp, align2d) buffers of those shapes to write instead of new tensors (a captured frame's pose)."""
     ref = srt if srt is not None else theta_in
     if ref is None:
         raise ValueError("pose_theta: srt or theta_in is required")
@@ -659,9 +661,16 @@ def pose_theta(srt: Optional[torch.Tensor], source_theta: Optional[torch.Tensor]
         raise ValueError(f"pose_theta: theta_in must be (N,4,4), got {tuple(theta_in.shape)}")
     if smooth_state is not None and tuple(smooth_state.shape) != (3, 4):
         raise ValueError(f"pose_theta: smooth_state must be (3,4), got {tuple(smooth_state.shape)}")
-    theta = torch.empty((N, 4, 4), dtype=torch.float32, device=dev)
-    warp = torch.empty((N, 3, 4), dtype=torch.float32, device=dev)
-    align = torch.empty((N, 2, 3), dtype=torch.float32, device=dev)
+    if out is None:
+        theta = torch.empty((N, 4, 4), dtype=torch.float32, device=dev)
+        warp = torch.empty((N, 3, 4), dtype=torch.float32, device=dev)
+        align = torch.empty((N, 2, 3), dtype=torch.float32, device=dev)
+    else:
+        theta, warp, align = out
+        for t, shp in zip(out, ((N, 4, 4), (N, 3, 4), (N, 2, 3))):
+            _chk(t)
+            if tuple(t.shape) != shp:
+                raise ValueError(f"pose_theta: out must be (N,4,4), (N,3,4), (N,2,3), got {[tuple(o.shape) for o in out]}")
     d = pose_desc(N, _p(srt), _p(source_theta), _p(theta), _p(warp), _p(align), _p(theta_in), _p(smooth_state), mix=mix,
                   invert_warp=invert_warp, mix_old=mix_old, smooth_init=smooth_init, smooth_momentum=smooth_momentum)
     L.call("emo_pose_theta", C.byref(d), _stream())
