@@ -3,8 +3,9 @@ plan it names, and the table as a whole reaches every configuration of the plann
 case against float64).
 
 A case is a convolution (shape + options of ops.conv_igemm) and the plan class it is meant to reach at 132 SMs (H100 SXM):
-"<kernel instantiation> BN<N tile> <main loop> <finish>", main loop "rr2" / "rr3" (row reuse with an A ring of 2 / 3 halo
-tiles) or "tap" (one {A, B} stage per tap), finish as emo_conv_plan_info.finish (lib.CONV_FINISH)."""
+"<kernel instantiation> BN<N tile> <main loop> <finish>[ 3-D]", main loop "rr2" / "rr3" (row reuse with an A ring of 2 / 3
+halo tiles) or "tap" (one {A, B} stage per tap), finish as emo_conv_plan_info.finish (lib.CONV_FINISH), " 3-D" for inputs of
+depth > 1 (plan_class): a 2-D case does not sweep the depth halo, padding and tiles of a 3-D launch."""
 from __future__ import annotations
 
 import math
@@ -90,7 +91,8 @@ CASES = [
     Case("ps<64,2> BN64 rr3 none", 64, 64, (48, 40), upconv=True, post_add=True, stats=True),
     # fp16 two planes, KC = 64
     Case("f16<64,2> BN128 rr2 none", 64, 128, (96, 96), planes=H2, residual=True, stats=True),
-    Case("f16<64,2> BN128 rr2 apply", 64, 256, (4, 16, 80), planes=H2, post=True, stats=True),
+    Case("f16<64,2> BN128 rr2 apply 3-D", 64, 256, (4, 16, 80), planes=H2, post=True, stats=True),
+    Case("f16<64,2> BN128 rr2 apply", 128, 256, (64, 80), planes=H2, post=True, stats=True),
     Case("f16<64,2> BN128 tap none", 64, 128, (96, 96), k=1, planes=H2, post_add=True, stats=True),
     Case("f16<64,2> BN128 tap finalize", 512, 128, (4, 4), k=1, planes=H2, out_nchw=True),
     Case("f16<64,2> BN128 tap finalize+apply", 128, 128, (32, 32), planes=H2, post=True, stats=True),
@@ -100,20 +102,35 @@ CASES = [
     Case("f16<64,2> BN96 tap none", 64, 192, (96, 40), k=1, planes=H2, stats=True),
     Case("f16<64,2> BN64 rr3 none", 64, 64, (96, 96), planes=H2, residual=True, stats=True),
     Case("f16<64,2> BN64 rr3 apply", 64, 64, (96, 96), planes=H2, post=True, stats=True),
-    Case("f16<64,2> BN64 tap none", 128, 64, (4, 64, 64), k=1, planes=H2),
+    Case("f16<64,2> BN64 tap none 3-D", 128, 64, (4, 64, 64), k=1, planes=H2),
     Case("f16<64,2> BN64 tap finalize+apply", 64, 64, (64, 64), planes=H2, post=True, stats=True),
     Case("f16<64,2> BN64 tap post", 64, 64, (32, 32), planes=H2, post=True, stats=True),
-    Case("f16<64,2> BN32 rr3 apply", 64, 32, (8, 64, 64), planes=H2, post=True, stats=True),
-    Case("f16<64,2> BN32 tap none", 64, 32, (8, 64, 64), k=1, planes=H2, residual=True),
+    Case("f16<64,2> BN32 rr3 apply 3-D", 64, 32, (8, 64, 64), planes=H2, post=True, stats=True),
+    Case("f16<64,2> BN32 tap none 3-D", 64, 32, (8, 64, 64), k=1, planes=H2, residual=True),
+    Case("f16<64,2> BN32 tap none", 64, 256, (64, 64), k=1, planes=H2, split_k=False, stats=True),
     Case("f16<64,2> BN32 tap apply", 64, 32, (96, 96), k=1, planes=H2, post=True, stats=True),
     Case("f16<64,2> BN16 tap none", 256, 512, (8, 8), k=1, stride=2, planes=H2, residual=True),
     Case("f16<64,2> BN16 tap apply", 64, 64, (32, 32), k=1, planes=H2, post=True, stats=True),
     # fp16 two planes, KC = 32
-    Case("f16<32,2> BN96 rr3 none", 96, 96, (4, 64, 64), planes=H2, residual=True, stats=True),
-    Case("f16<32,2> BN96 rr3 apply", 96, 96, (4, 64, 64), planes=H2, post=True, stats=True),
-    Case("f16<32,2> BN96 tap none", 96, 96, (4, 64, 64), k=1, planes=H2, out_nchw=True),
-    Case("f16<32,2> BN32 rr3 none", 32, 32, (8, 64, 64), planes=H2, residual=True),
+    Case("f16<32,2> BN96 rr3 none 3-D", 96, 96, (4, 64, 64), planes=H2, residual=True, stats=True),
+    Case("f16<32,2> BN96 rr3 apply 3-D", 96, 96, (4, 64, 64), planes=H2, post=True, stats=True),
+    Case("f16<32,2> BN96 tap none 3-D", 96, 96, (4, 64, 64), k=1, planes=H2, out_nchw=True),
+    Case("f16<32,2> BN32 rr3 none 3-D", 32, 32, (8, 64, 64), planes=H2, residual=True),
     Case("f16<32,2> BN16 rr3 none", 32, 3, (4, 16), planes=H2, split_k=False, post_add=True),
+    # the 3-D layers of stage 1 in exact mode (Cin / Cout as the model's): volume blocks, U-Net, warp generator.  A 3-D per-tap
+    # case tiles depth (td = 2 on 8 x 8 slices) with a depth the tile does not divide; row reuse keeps a tile in one depth
+    # slice (td = 1), so its cases take an odd depth, whose first and last output slices read the depth padding.
+    Case("f16<64,2> BN128 rr2 none 3-D", 384, 384, (5, 32, 32), planes=H2, residual=True, stats=True),
+    Case("f16<64,2> BN128 tap none 3-D", 192, 384, (45, 8, 8), k=1, planes=H2, split_k=False),
+    Case("f16<64,2> BN128 tap finalize 3-D", 256, 256, (7, 8, 8), planes=H2, residual=True, stats=True),
+    Case("f16<64,2> BN128 tap finalize+apply 3-D", 512, 256, (5, 8, 8), planes=H2, post=True, stats=True),
+    Case("f16<64,2> BN96 rr3 none 3-D", 192, 192, (5, 32, 32), planes=H2, residual=True, stats=True),
+    Case("f16<64,2> BN96 rr3 apply 3-D", 384, 192, (5, 32, 32), planes=H2, post=True, stats=True),
+    Case("f16<64,2> BN96 tap none 3-D", 384, 192, (65, 8, 8), k=1, planes=H2, split_k=False),
+    Case("f16<64,2> BN64 rr3 none 3-D", 64, 64, (9, 32, 32), planes=H2, residual=True, stats=True),
+    Case("f16<64,2> BN64 rr3 apply 3-D", 128, 64, (9, 32, 32), planes=H2, post=True, stats=True),
+    # the warp generator's head: tanh, then the identity grid added
+    Case("f16<32,2> BN16 rr3 none 3-D", 32, 3, (5, 16, 24), planes=H2, split_k=False, act=TANH, post_add=True),
 
     # ---- configurations the models do not reach today ----
     # the other wgmma N widths (bf16 and fp16 have one instruction form per width)
@@ -125,10 +142,10 @@ CASES = [
     Case("conv<64,2> BN16 tap none", 64, 16, (8, 16), k=1, split_k=False, stats=True, G=16),
     # three planes (fp32-faithful bf16)
     Case("conv<64,3> BN64 rr2 none", 64, 64, (96, 96), planes=B3, residual=True, stats=True),
-    Case("conv<32,3> BN128 tap finalize", 512, 256, (8, 8, 8), planes=B3, residual=True, stats=True),
-    Case("conv<64,3> BN16 tap none", 64, 64, (16, 16, 16), k=3, stride=2, planes=B3, split_k=False, residual=True, stats=True),
-    Case("conv<32,3> BN96 rr3 none", 64, 96, (4, 48, 48), planes=B3, residual=True, stats=True),
-    Case("conv<32,3> BN16 tap none", 96, 96, (8, 8, 8), planes=B3, split_k=False, residual=True, stats=True),
+    Case("conv<32,3> BN128 tap finalize 3-D", 512, 256, (8, 8, 8), planes=B3, residual=True, stats=True),
+    Case("conv<64,3> BN16 tap none 3-D", 64, 64, (16, 16, 16), k=3, stride=2, planes=B3, split_k=False, residual=True, stats=True),
+    Case("conv<32,3> BN96 rr3 none 3-D", 64, 96, (4, 48, 48), planes=B3, residual=True, stats=True),
+    Case("conv<32,3> BN16 tap none 3-D", 96, 96, (8, 8, 8), planes=B3, split_k=False, residual=True, stats=True),
     # row reuse with KC = 32 although Cin % 64 == 0 (a 64-channel halo tile does not fit next to the B ring)
     Case("conv<32,2> BN128 rr3 none", 64, 1024, (2, 256), N=4, residual=True),
     Case("f16<32,2> BN128 rr3 none", 64, 1024, (2, 256), N=4, planes=H2, residual=True),
@@ -140,19 +157,26 @@ CASES = [
     # items > grid in the per-tap loop, ragged boxes, odd Cout on the scalar path, explicit accumulation chunks
     Case("conv<64,2> BN16 tap none", 64, 5, (96, 200), k=1, residual=False, stats=True, G=5, acc=6),
     Case("conv<64,3> BN16 tap none", 64, 7, (40, 72), k=3, stride=2, planes=B3, split_k=False, out_nchw=True, acc=30, N=2),
-    Case("f16<64,2> BN16 tap none", 64, 12, (20, 20, 20), k=3, stride=2, planes=H2, split_k=False, residual=True, stats=True, G=4, acc=9),
-    Case("conv<32,3> BN128 tap none", 96, 256, (24, 24, 24), k=1, planes=B3, post_add=True),
+    Case("f16<64,2> BN16 tap none 3-D", 64, 12, (20, 20, 20), k=3, stride=2, planes=H2, split_k=False, residual=True, stats=True, G=4, acc=9),
+    Case("conv<32,3> BN128 tap none 3-D", 96, 256, (24, 24, 24), k=1, planes=B3, post_add=True),
     Case("f16<32,2> BN16 tap none", 32, 13, (72, 72), k=1, planes=H2, residual=True, acc=3),
     Case("conv<64,2> BN128 rr2 none", 64, 384, (80, 80), residual=True, res_shift=1, post_add=True, acc=40),
     Case("ps<64,2> BN128 rr2 none", 128, 256, (40, 56), upconv=True, residual=True, res_shift=1, stats=True, acc=36),
 ]
 
 
-def plan_class(info) -> str:
+def plan_class(info, depth: int) -> str:
+    """plan class of a convolution whose input has `depth` slices: " 3-D" follows the class of a volume (depth > 1), whose
+    tiles meet the depth halo, depth padding and depth tiles that a 2-D map never reaches"""
     from emoportraits_b200 import lib as L
 
     loop = f"rr{info.sa}" if info.yreuse else "tap"
-    return f"{L.CONV_KERNELS[info.kernel]} BN{info.BN} {loop} {L.CONV_FINISH[info.finish]}"
+    return f"{L.conv_kernel_name(info.kernel)} BN{info.BN} {loop} {L.CONV_FINISH[info.finish]}" + (" 3-D" if depth > 1 else "")
+
+
+def depth(c: Case) -> int:
+    """input depth of a case (1 for a 2-D map)"""
+    return c.sp[0] if len(c.sp) == 3 else 1
 
 
 # ------------------------------------------------------------------------------------------------------------------

@@ -21,9 +21,13 @@ ROOT = pathlib.Path(__file__).resolve().parents[1]
 TABLE = pathlib.Path(__file__).resolve().parent / "model_conv_launches.json"
 SM_COUNT = 132   # H100 SXM
 
-# stage 1: source pass + driver pass at S^2; stage 2: one forward at S^2 of a batch of B frames
+# stage 1: source pass + driver pass at S^2; stage 2: one forward at S^2 of a batch of B frames.  "srcfast" is stage 1 with
+# the source pass on one fp16 plane (InferenceWrapper(source_precision="fast")); its driver pass is the exact mode's.  The
+# tables list launches in order of first appearance: a configuration added at the end leaves the earlier entries in place.
 CONFIGS = ("s1-256-exact", "s1-256-fast", "s1-512-exact", "s1-512-fast",
-           "s2-512-b1-exact", "s2-512-b1-fast", "s2-1024-b4-exact", "s2-1024-b4-fast", "s2-1024-b16-exact", "s2-1024-b16-fast")
+           "s2-512-b1-exact", "s2-512-b1-fast", "s2-1024-b4-exact", "s2-1024-b4-fast", "s2-1024-b16-exact", "s2-1024-b16-fast",
+           "s1-256-srcfast", "s1-512-srcfast")
+PRECISIONS = dict(s1=("exact", "fast", "srcfast"), s2=("exact", "fast"))   # the last field of a configuration, per stage
 
 
 def _split(desc_type, d):
@@ -81,6 +85,8 @@ def run(config: str, hook) -> None:
             from emoportraits_b200.config import shipped_config
             from emoportraits_b200.infer import Model
 
+            if precision == "srcfast":   # what InferenceWrapper(source_precision="fast") passes
+                precision = dict(Model.PRESETS["exact"], **Model.SOURCE_FAST)
             cfg = shipped_config(int(size))
             model = Model(cfg, synthetic_state_dict(cfg, 0), synthetic_head_pose_state_dict(0), "cpu", precision=precision)
             x = torch.rand(1, 3, int(size), int(size))
@@ -146,7 +152,7 @@ if __name__ == "__main__":
         TABLE.write_text(dumps(rows))
         print(f"{TABLE.name}: {len(rows)} distinct launches")
     else:
-        unknown = [a for a in args if a.split("-")[0] not in ("s1", "s2")]
+        unknown = [a for a in args if a.split("-")[-1] not in PRECISIONS.get(a.split("-")[0], ())]
         if not args or unknown:
             sys.exit(f"usage: {sys.argv[0]} --write | CONFIG... (e.g. {' '.join(CONFIGS[:2])}); unknown: {unknown}")
         print("LAUNCHES " + json.dumps(table(args)))

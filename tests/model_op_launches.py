@@ -182,7 +182,7 @@ if __name__ == "__main__":
         TABLE.write_text(dumps(rows))
         print(f"{TABLE.name}: {len(rows)} distinct launches")
     else:
-        unknown = [a for a in args if a.split("-")[0] not in ("s1", "s2")]
+        unknown = [a for a in args if a.split("-")[-1] not in MCL.PRECISIONS.get(a.split("-")[0], ())]
         if not args or unknown:
             sys.exit(f"usage: {sys.argv[0]} --write | CONFIG... (e.g. {' '.join(CONFIGS[:2])}); unknown: {unknown}")
         print("LAUNCHES " + json.dumps(table(args)))

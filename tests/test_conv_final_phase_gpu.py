@@ -64,7 +64,7 @@ def test_final_phase_against_float64(ops, c):
     st = torch.zeros((c.N, c.G, 2), dtype=torch.float64, device="cuda") if c.stats else None
     a, pw, kw = CP.conv_args(c, ops, x, w, b, res, pa, stats=st, out=out)
     info = ops.conv_plan(a, pw, **kw)
-    assert info.ksplit == 1 and L.CONV_FINISH[info.finish] == "none", CP.plan_class(info)
+    assert info.ksplit == 1 and L.CONV_FINISH[info.finish] == "none", CP.plan_class(info, CP.depth(c))
 
     ops.conv_igemm(a, pw, **kw)
     torch.cuda.synchronize()
@@ -72,7 +72,7 @@ def test_final_phase_against_float64(ops, c):
     assert torch.isnan(buf[numel:]).all(), "write past the end of the output tensor"
     assert not torch.isnan(out).any(), f"{int(torch.isnan(out).sum())} output elements never written"
     e = (_to_ncdhw(c, out).double() - ref).abs().max().item()
-    assert e < TOL * max(1.0, scale), (CP.plan_class(info), e, scale)
+    assert e < TOL * max(1.0, scale), (CP.plan_class(info, CP.depth(c)), e, scale)
     if st is not None:
         r = ref.reshape(c.N, c.G, -1)
         count = r.shape[-1]
@@ -80,4 +80,4 @@ def test_final_phase_against_float64(ops, c):
         msq = (r * r).mean(-1)
         d_msq = ((st[..., 1] / count - msq).abs() / msq).max().item()
         assert d_mean < 1e-6 * max(1.0, scale) and d_msq < 1e-5, (d_mean, d_msq)
-    print(f"\n[{c.id}] {CP.plan_class(info)}: max-abs {e:.2e} (scale {scale:.2f})")
+    print(f"\n[{c.id}] {CP.plan_class(info, CP.depth(c))}: max-abs {e:.2e} (scale {scale:.2f})")

@@ -4,7 +4,8 @@
     split-K finish paths, ragged boxes, padded / odd Cout, both statistics branches, ...): a later change of the planner's
     heuristics that leaves a configuration unchecked by tests/test_conv_plan_gpu.py fails here, naming it;
   * every convolution the shipped models issue (stage 1 at 256 and 512, stage 2 at 512 and 1024: recorded in EMO_DRY_RUN
-    mode) passes the planner's checks and falls in a plan class the case table covers."""
+    mode) passes the planner's checks and falls in a plan class the case table covers with a case of its dimension (a
+    " 3-D" class for inputs of depth > 1)."""
 import json
 import os
 import pathlib
@@ -55,7 +56,7 @@ def test_header_enums_match_the_binding():
 
 
 def test_cases_reach_their_plan_class(plans):
-    bad = [(c.id, c.want, CP.plan_class(p)) for c, p in plans if CP.plan_class(p) != c.want]
+    bad = [(c.id, c.want, CP.plan_class(p, CP.depth(c))) for c, p in plans if CP.plan_class(p, CP.depth(c)) != c.want]
     assert not bad, "\n".join(f"{i}: wants {w}, plans {g}" for i, w, g in bad)
 
 
@@ -170,7 +171,7 @@ def test_model_layers_fall_in_swept_plan_classes(model):
     for v in rows:
         d = v["conv"]
         info = L.ConvPlanInfo(**v["plan"])
-        cls = CP.plan_class(info)
+        cls = CP.plan_class(info, d["Din"])
         opts = " ".join(sorted(set(v["conv_ptrs"]) - {"a_hi", "a_lo", "a_lo2", "w_hi", "w_lo", "w_lo2", "out", "splitk_ws"}))
         name = f"{_old_key(v)} p{d['ph']}{d['pw']} rs{d['res_shift']} act{d['act']} [{opts}]"
         print(f"  {name:90s} {cls:36s} ksplit {info.ksplit:2d} grid {info.grid:3d}")

@@ -48,9 +48,10 @@ def test_conv_case_against_float64(ops, c):
     info = ops.conv_plan(a, pw, **kw)
     sms = torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
     if sms == CP.SM_COUNT:
-        assert CP.plan_class(info) == c.want, (CP.plan_class(info), c.want)
+        assert CP.plan_class(info, CP.depth(c)) == c.want, (CP.plan_class(info, CP.depth(c)), c.want)
     else:
-        print(f"\n[{c.id}] {sms} SMs, not {CP.SM_COUNT}: plan class {CP.plan_class(info)} not checked against {c.want}")
+        print(f"\n[{c.id}] {sms} SMs, not {CP.SM_COUNT}: plan class {CP.plan_class(info, CP.depth(c))} not checked against "
+              f"{c.want}")
     finish = L.CONV_FINISH[info.finish]
 
     got = ops.conv_igemm(a, pw, **kw)
@@ -58,7 +59,7 @@ def test_conv_case_against_float64(ops, c):
     ref, scale = CP.reference(c, x, w, b, res, pa)
     assert torch.isnan(buf[numel:]).all(), "write past the end of the output tensor"
     kern = L.CONV_KERNELS[info.kernel]
-    msg = f"\n[{c.id}] {CP.plan_class(info)} ksplit {info.ksplit} grid {info.grid}:"
+    msg = f"\n[{c.id}] {CP.plan_class(info, CP.depth(c))} ksplit {info.ksplit} grid {info.grid}:"
     if finish != "post":      # the fused split-K post kernel writes the post-op's output only
         assert not torch.isnan(out).any(), f"{int(torch.isnan(out).sum())} output elements never written"
         err = (_to_ncdhw(c, out).double() - ref).abs()

@@ -12,6 +12,8 @@ import ctypes as C
 import pytest
 import torch
 
+import conv_plan_cases as CP
+
 SOURCE_NETS = ("LocalEncoder", "VolumeSource", "Unet3D")
 
 
@@ -125,7 +127,7 @@ def test_fast_source_plans_every_source_conv_on_one_plane(dry, monkeypatch, size
     # every one-plane plan written by an apply / post-op in the source networks is one fp16 plane of x16
     applies = [dict(f) for _, n, f, _ in src if n == "emo_apply"]
     assert applies and all(a["plane_fp16"] == 1 and a["plane_scale"] == ops.F16_ACT_SCALE and not a["out_lo"] for a in applies)
-    classes = [TF.plan_class(info, d.Din) for _, info, d in convs]
+    classes = [CP.plan_class(info, d.Din) for _, info, d in convs]
     print(f"\n[fast source pass @{size}^2] {len(convs)} convolutions: "
           + ", ".join(f"{k} x{classes.count(k)}" for k in sorted(set(classes))))
     unswept = sorted(set(classes) - _swept_classes())
@@ -162,8 +164,8 @@ def test_gpu_cases_reach_their_plan_class(dry):
         st = torch.zeros((1, TF.G, 2), dtype=torch.float64) if c.stats else None
         a, pw, kw = TF.conv_args(c, ops, x, w, b, res, st)
         info = ops.conv_plan(a, pw, sm_count=132, **kw)
-        if TF.plan_class(info, c.sp[0]) != want or info.NP != 1:
-            bad.append((c.id, want, TF.plan_class(info, c.sp[0])))
+        if CP.plan_class(info, c.sp[0]) != want or info.NP != 1:
+            bad.append((c.id, want, CP.plan_class(info, c.sp[0])))
     assert not bad, bad
     a, pw, kw = TF.conv_args(TF.DEPTH_CASE[1], ops, *TF.make(TF.DEPTH_CASE[1], ops, "cpu"),
                              stats=torch.zeros((1, TF.G, 2), dtype=torch.float64))

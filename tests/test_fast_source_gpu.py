@@ -28,6 +28,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+import conv_plan_cases as CP
 from oracle import frames as FR
 
 pytestmark = pytest.mark.gpu
@@ -70,8 +71,9 @@ class Case:
         return tuple((i + 2 * p - k) // s + 1 for i, k, p, s in zip(self.sp, self.k, self.padding, self.strides))
 
 
-# plan class at 132 SMs (plan_class(): "<kernel> BN<N tile> <main loop> <finish>", " 3-D" for inputs of depth > 1) -> case (the layer each
-# stands for).  The 3-D shapes are the model's with fewer depth slices or rows where that keeps the plan class.
+# plan class at 132 SMs (conv_plan_cases.plan_class(): "<kernel> BN<N tile> <main loop> <finish>", " 3-D" for inputs of
+# depth > 1) -> case (the layer each stands for).  The 3-D shapes are the model's with fewer depth slices or rows where that
+# keeps the plan class.
 CASES = [
     ("h1<32,1> BN96 rr3 none 3-D", Case(96, 96, (16, 64, 64), residual=True, stats=True)),         # VolumeSource, second conv
     ("h1<32,1> BN96 rr3 apply 3-D", Case(96, 96, (16, 64, 64), post=True, stats=True)),            # VolumeSource, first conv
@@ -95,14 +97,6 @@ DEPTH_CASE = ("h1<32,1> BN96 tap finalize 3-D", Case(96, 96, (4, 8, 8), residual
 def ops():
     from emoportraits_b200 import ops as o
     return o
-
-
-def plan_class(info, depth):
-    """plan class of a convolution whose input has `depth` slices"""
-    from emoportraits_b200 import lib as L
-
-    loop = f"rr{info.sa}" if info.yreuse else "tap"
-    return f"{L.conv_kernel_name(info.kernel)} BN{info.BN} {loop} {L.CONV_FINISH[info.finish]}" + (" 3-D" if depth > 1 else "")
 
 
 def make(c: Case, ops, device="cuda"):
@@ -199,7 +193,7 @@ def check_case(ops, want, c, depth_tiled=False):
     assert info.NP == 1 and info.fp16 == 1
     assert (info.td > 1) == depth_tiled, info.td
     if torch.cuda.get_device_properties(0).multi_processor_count == 132:
-        assert plan_class(info, c.sp[0]) == want, (plan_class(info, c.sp[0]), want)
+        assert CP.plan_class(info, c.sp[0]) == want, (CP.plan_class(info, c.sp[0]), want)
     outs, guards = run_guarded(c, ops, a, pw, kw)
     for name, g in guards.items():
         assert torch.isnan(g.float()).all(), f"{name}: write past the end of the output"

@@ -1,9 +1,9 @@
 """CPU checks of the table of model convolution launches (tests/model_conv_launches.py, replayed on the GPU by
 tests/test_model_conv_launches_gpu.py):
-  * recorded afresh in EMO_DRY_RUN mode, the launches of the ten configurations equal the committed table, so that a model
-    change fails here until the table is regenerated;
-  * no launch is refused and every launch plans, at 132 SMs, in a class that a GPU case sweeps (tests/conv_plan_cases.py and
-    the fast-mode case lists);
+  * recorded afresh in EMO_DRY_RUN mode, the launches of the twelve configurations (model_conv_launches.CONFIGS) equal the
+    committed table, so that a model change fails here until the table is regenerated;
+  * no launch is refused and every launch plans, at 132 SMs, in a class that a GPU case of the same dimension (2-D or 3-D)
+    sweeps (tests/conv_plan_cases.py and the fast-mode case lists);
   * the replay's float64 references (a sum over taps of shifted-activation matrix products, and its sub-pixel form) equal
     torch's float64 convolutions."""
 import json
@@ -48,12 +48,16 @@ def test_committed_table_is_current(fresh):
 
 def _swept_classes():
     import test_fast_decoder_gpu as TD
+    import test_fast_source_gpu as TF
     import test_fast_stage2_gpu as TS
 
-    return {c.want for c in CP.CASES} | {w for w, _ in TD.CASES} | {w for w, _ in TS.CASES}
+    return ({c.want for c in CP.CASES} | {w for w, _ in TD.CASES} | {w for w, _ in TS.CASES} | {w for w, _ in TF.CASES}
+            | {TF.DEPTH_CASE[0]})
 
 
 def test_every_launch_plans_in_a_swept_class(fresh):
+    """a class is "<kernel> BN<n> <loop> <finish>", with " 3-D" for inputs of depth > 1: a 2-D case does not sweep a 3-D
+    launch's depth halo, padding and tiles, nor a 3-D case a 2-D launch's"""
     from emoportraits_b200 import lib as L
 
     refused = [(r["conv"], r["err"]) for r in fresh if r["rc"] != 0]
@@ -61,13 +65,11 @@ def test_every_launch_plans_in_a_swept_class(fresh):
     swept = _swept_classes()
     classes = {}
     for r in fresh:
-        info = L.ConvPlanInfo(**r["plan"])
-        loop = f"rr{info.sa}" if info.yreuse else "tap"
-        cls = f"{L.conv_kernel_name(info.kernel)} BN{info.BN} {loop} {L.CONV_FINISH[info.finish]}"
+        cls = CP.plan_class(L.ConvPlanInfo(**r["plan"]), r["conv"]["Din"])
         classes.setdefault(cls, []).append(r)
     print(f"\n[model conv launches] {len(classes)} plan classes at {MCL.SM_COUNT} SMs")
     for cls, rows in sorted(classes.items()):
-        print(f"  {cls:36s} {len(rows):4d}")
+        print(f"  {cls:40s} {len(rows):4d}")
     unswept = sorted(set(classes) - swept)
     assert not unswept, f"model launches in plan classes no GPU case sweeps: {unswept}"
 

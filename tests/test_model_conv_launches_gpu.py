@@ -1,5 +1,6 @@
 """GPU replay of every implicit-GEMM convolution the shipped models launch (tests/model_conv_launches.json: stage 1 at 256^2
-and 512^2, stage 2 at 512^2 batch 1 and 1024^2 batch 4 and 16, exact and fast), at its real shape, against float64.
+and 512^2 in exact mode, fast mode and with the fast source pass, stage 2 at 512^2 batch 1 and 1024^2 batch 4 and 16, exact
+and fast), at its real shape, against float64.
 
 Each launch is rebuilt from its recorded emo_conv_desc / emo_apply_desc scalars and called through lib.call, so the test runs
 exactly the fields the model passed.  Operands are seeded; every output (the convolution's, the post-op's fp32 tensor and

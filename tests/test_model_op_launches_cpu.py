@@ -1,8 +1,8 @@
 """CPU checks of the table of model non-convolution launches (tests/model_op_launches.py, replayed on the GPU by
 tests/test_model_op_launches_gpu.py):
-  * recorded afresh in EMO_DRY_RUN mode, the launches of the ten configurations (stage 1 at 256^2 and 512^2, stage 2 at 512^2
-    batch 1 and 1024^2 batch 4 and 16, each in exact and fast mode) equal the committed table, so that a model change fails
-    here until the table is regenerated;
+  * recorded afresh in EMO_DRY_RUN mode, the launches of the twelve configurations (stage 1 at 256^2 and 512^2 in exact
+    mode, fast mode and with the fast source pass; stage 2 at 512^2 batch 1 and 1024^2 batch 4 and 16, each in exact and fast
+    mode) equal the committed table, so that a model change fails here until the table is regenerated;
   * every launch, and the post-op of every model convolution (tests/model_conv_launches.json), falls in a variant class that a
     case of tests/op_cases.py checks against float64;
   * the wrapper-boundary list names lines that exist, and the mask helpers, run on host tensors, issue exactly its launches.
